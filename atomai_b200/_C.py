@@ -15,8 +15,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libatomai_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
-           "selftest.cu", "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo",
+           "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 ACT_LRELU = 0
@@ -29,9 +29,9 @@ WMODE_DGRAD = 1
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into libatomai_b200.so (in-tree)."""
+    """Compile every CUDA source for sm_90a into libatomai_b200.so (in-tree)."""
     srcs = [os.path.join(CSRC, s) for s in SOURCES]
-    deps = srcs + [os.path.join(CSRC, "common.cuh"),
+    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "wgmma.cuh"),
                    os.path.join(_HERE, "..", "include", "atomai_b200.h")]
     if not force and os.path.exists(LIB_PATH):
         t = os.path.getmtime(LIB_PATH)
@@ -125,10 +125,7 @@ SIGNATURES = {
     "atomai_b200_p2p_allreduce": (_i, [_vp, _vp, _i, _i, C.c_uint64, _vp, _i, _vp]),
     "atomai_b200_p2p_bn_finalize": (_i, [_vp, _vp, _i, _i, C.c_uint64, _vp, _i, _d, _vp, _vp, _vp,
                                          _vp, _f, _f, _vp, _vp, _vp, _vp, _vp]),
-    "atomai_b200_umma_rate": (_i, [_i, _i, _i, _i, _vp, _vp]),
     "atomai_b200_selftest_tma": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp]),
-    "atomai_b200_selftest_sw128": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
-    "atomai_b200_selftest_umma": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp]),
 }
 
 _lib = None

@@ -3,6 +3,10 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <map>
+#include <mutex>
+#include <utility>
+
 #include "common.cuh"
 
 // implemented in conv_tc.cu / conv_simt.cu / wgrad_tc.cu
@@ -47,14 +51,50 @@ int ab_optin_smem(const void* func, int bytes, unsigned char* done) {
 int ab_num_sms() {
   static int sms[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (sms[dev] == 0) {
     int v = 0;
     if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0)
-      v = 148;
+      v = 132;
     sms[dev] = v;
   }
   return sms[dev];
+}
+
+// One workspace per (device, stream): launches on one stream run in order, so the slots and
+// tickets of consecutive launches never overlap; launches on different streams get different
+// workspaces and may run concurrently.
+int ab_ordered_ws(cudaStream_t stream, int64_t n_doubles, int groups, Ordered* out) {
+  constexpr int kMaxGroups = 4096;
+  struct Ws {
+    double* slots = nullptr;
+    int64_t cap = 0;
+    unsigned* tickets = nullptr;
+  };
+  static std::mutex mu;
+  static std::map<std::pair<int, cudaStream_t>, Ws> table;
+  int dev = 0;
+  AB_CUDA(cudaGetDevice(&dev));
+  AB_CHECK(groups >= 1 && groups <= kMaxGroups && n_doubles >= 0,
+           "ordered-sum workspace: %d groups", groups);
+  std::lock_guard<std::mutex> lock(mu);
+  Ws& w = table[std::make_pair(dev, stream)];
+  if (!w.tickets) {
+    AB_CUDA(cudaMalloc(&w.tickets, kMaxGroups * sizeof(unsigned)));
+    AB_CUDA(cudaMemsetAsync(w.tickets, 0, kMaxGroups * sizeof(unsigned), stream));
+  }
+  if (n_doubles > w.cap) {
+    // cudaFree waits for the device, so no launch still reads the old buffer
+    const int64_t want = n_doubles > 2 * w.cap ? n_doubles : 2 * w.cap;
+    if (w.slots) AB_CUDA(cudaFree(w.slots));
+    w.slots = nullptr;
+    w.cap = 0;
+    AB_CUDA(cudaMalloc(&w.slots, want * sizeof(double)));
+    w.cap = want;
+  }
+  out->slots = w.slots;
+  out->ticket = w.tickets;
+  return 0;
 }
 
 int ab_make_srcset(const ab_conv_t* d, SrcSet* out) {
@@ -89,7 +129,7 @@ int ab_make_srcset(const ab_conv_t* d, SrcSet* out) {
 
 extern "C" {
 
-const char* atomai_b200_version(void) { return "atomai_b200 0.1.0 (sm_100a)"; }
+const char* atomai_b200_version(void) { return "atomai_b200 0.1.0 (sm_90a)"; }
 const char* atomai_b200_last_error(void) { return g_err; }
 
 int atomai_b200_device_ok(int device) {
@@ -98,7 +138,7 @@ int atomai_b200_device_ok(int device) {
     ab_set_error("cannot query device %d", device);
     return 0;
   }
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 int64_t atomai_b200_prep_weights_elems(int Cout, int Cin, int ks_h, int ks_w, int mode, int math) {
@@ -123,7 +163,7 @@ int atomai_b200_conv_fwd(const ab_conv_t* d, const float* w_prepped, const float
   AB_CHECK(d->out_nchw || ld_y >= d->Cout, "conv_fwd: ld_y=%d < Cout=%d", ld_y, d->Cout);
   if (d->math == AB_MATH_TF32 || d->math == AB_MATH_TF32X3) {
     AB_CHECK(ab_conv_tc_supported(d),
-             "conv_fwd: shape not supported by the tcgen05 path (need C%%8==0, Cout%%16==0, "
+             "conv_fwd: shape not supported by the tensor-core path (need C%%8==0, Cout%%16==0, "
              "16<=Cout<=256, 16B-aligned sources); use AB_MATH_FP32");
     return ab_conv_tc_fwd(d, w_prepped, bias, y, ld_y, stats, (cudaStream_t)stream);
   }
@@ -139,7 +179,7 @@ int atomai_b200_conv_supported(const ab_conv_t* d, int which) {
 int atomai_b200_conv_info(const ab_conv_t* d, int* grid, int* block, int* smem_bytes) {
   AB_CHECK(d && grid && block && smem_bytes, "conv_info: null pointer");
   AB_CHECK((d->math == AB_MATH_TF32 || d->math == AB_MATH_TF32X3) && ab_conv_tc_supported(d),
-           "conv_info: tcgen05 path only");
+           "conv_info: tensor-core path only");
   return ab_conv_tc_info(d, grid, block, smem_bytes);
 }
 
@@ -148,7 +188,7 @@ int atomai_b200_conv_wgrad(const ab_conv_t* d, const float* dy, int ld_dy, float
   AB_CHECK(d && dy && dw_oihw, "conv_wgrad: null pointer");
   AB_CHECK(ld_dy >= d->Cout, "conv_wgrad: ld_dy=%d < Cout=%d", ld_dy, d->Cout);
   if (d->math == AB_MATH_TF32 || d->math == AB_MATH_TF32X3) {
-    AB_CHECK(ab_wgrad_tc_supported(d), "conv_wgrad: shape not supported by the tcgen05 path");
+    AB_CHECK(ab_wgrad_tc_supported(d), "conv_wgrad: shape not supported by the tensor-core path");
     return ab_conv_tc_wgrad(d, dy, ld_dy, dw_oihw, (cudaStream_t)stream);
   }
   AB_CHECK(d->math == AB_MATH_FP32, "conv_wgrad: math=%d", d->math);

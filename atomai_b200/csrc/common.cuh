@@ -1,6 +1,6 @@
-// common.cuh — error plumbing, PTX wrappers (mbarrier / bulk copy / tcgen05) and
+// common.cuh — error plumbing, PTX wrappers (mbarrier / bulk copy) and
 // the shared "source loader" used by every convolution-family kernel.
-// sm_100a only.  Test infrastructure lives elsewhere; this is product code.
+// sm_90a only.  Test infrastructure lives elsewhere; this is product code.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -83,8 +83,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 }
 // try_wait with a suspend-time hint: the hardware parks the thread until the phase completes (or the
 // hint expires) instead of returning at once, so a waiting warp does not hammer the shared-memory
-// pipe the tensor core reads its operands through (ncu, round 2: mbarrier polling was 12 % of the
-// L1 data-pipe wavefronts of conv_tc, next to 39 % of tcgen05 operand reads).
+// pipe the tensor core reads its operands through.
 __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -119,13 +118,26 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// The same bound without the diagnostic printf: a function call between wgmma issue and
+// wgmma.wait would make ptxas serialise the warpgroup MMAs.
+__device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
+  uint32_t spins = 0;
+  uint64_t t0 = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if ((++spins & 255u) == 0) {
+      const uint64_t now = global_timer_ns();
+      if (t0 == 0) t0 = now;
+      if (now - t0 > 20000000000ull) __trap();
+    }
+  }
+}
 __device__ __forceinline__ void prefetch_l2(const void* p) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma / bulk copies)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -151,136 +163,6 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// whole warp; writes the TMEM base address to *dst_smem
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], TF32 operands, fp32 accumulate; one thread issues.
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same with the descriptors split into 32-bit halves: only the low word (start address field)
-// changes between MMAs, so the issuing thread advances two 32-bit counters per MMA.
-__device__ __forceinline__ void umma_tf32_lh(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi,
-                                             uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::f16 (BF16 operands, fp32 accumulate), same split-descriptor form: the correction MMA of
-// the tf32x3 mode accumulates into the same TMEM tile as the kind::tf32 MMA before it.
-__device__ __forceinline__ void umma_bf16_lh(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi,
-                                             uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(tmem_d),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued MMAs of this thread -> one arrive on `bar` when they retire
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns; warp w may touch lanes 32*(w%4)..+31 only
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// UMMA shared-memory descriptor, SWIZZLE_NONE ("interleave") canonical layouts:
-//   K-major : ((8,m),(4,2)) : ((16B, SBO), (4B, LBO))   — 8-row core matrices of 16B rows
-//   MN-major: ((4,m),(8,k)) : ((4B, SBO), (16B, LBO))
-// Fields in 16-byte units; bit 46 = descriptor version 1 (Blackwell).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                              uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-// Same, with an explicit layout type (1 = SWIZZLE_128B_BASE32B, the only legal layout for
-// MN-major TF32 operands) and swizzle base offset.
-__device__ __forceinline__ uint64_t umma_desc_ex(uint32_t saddr, uint32_t lbo_bytes,
-                                                 uint32_t sbo_bytes, uint32_t layout_type,
-                                                 uint32_t base_offset) {
-  uint64_t d = umma_desc(saddr, lbo_bytes, sbo_bytes);
-  d |= (uint64_t)(base_offset & 7) << 49;
-  d |= (uint64_t)(layout_type & 7) << 61;
-  return d;
-}
-// byte-address swizzle of SWIZZLE_128B_BASE32B: 32 B chunk index ^= (128 B row index mod 4)
-__device__ __forceinline__ uint32_t swz128_32(uint32_t a) { return a ^ (((a >> 7) & 3u) << 5); }
-// Instruction descriptor, kind::tf32, fp32 accumulate.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_tf32(int M, int N, int a_mn_major,
-                                                             int b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;                        // D format: F32
-  d |= 2u << 7;                        // A format: TF32
-  d |= 2u << 10;                       // B format: TF32
-  d |= (uint32_t)(a_mn_major & 1) << 15;
-  d |= (uint32_t)(b_mn_major & 1) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
-}
-
-// Instruction descriptor, kind::f16 with BF16 operands (K = 16 per MMA), fp32 accumulate.
-__host__ __device__ __forceinline__ uint32_t umma_idesc_bf16(int M, int N, int a_mn_major,
-                                                             int b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;                        // D format: F32
-  d |= 1u << 7;                        // A format: BF16
-  d |= 1u << 10;                       // B format: BF16
-  d |= (uint32_t)(a_mn_major & 1) << 15;
-  d |= (uint32_t)(b_mn_major & 1) << 16;
-  d |= (uint32_t)(N >> 3) << 17;
-  d |= (uint32_t)(M >> 4) << 24;
-  return d;
-}
 // two floats -> packed bf16x2 (lo half = first argument), round to nearest even
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   uint32_t r;
@@ -442,3 +324,42 @@ __device__ __forceinline__ float load_src1(const SrcSet& S, int n, int h, int w,
 }
 
 int ab_make_srcset(const ab_conv_t* d, SrcSet* out);  // validates + converts (host)
+
+// ---------------------------------------------------------------- ordered cross-CTA sums
+// Run-to-run deterministic replacement for "one atomicAdd per CTA (or warp) and value": floating-
+// point addition is not associative, so sums whose order depends on which CTA finishes first
+// differ in the last bits from run to run, and training (Adam on gradients that are pure rounding,
+// e.g. a conv bias in front of BatchNorm) amplifies that.  Instead every contributing slot stores
+// its n partials; the last CTA to finish adds all slots in slot order and adds the result to dst.
+struct Ordered {
+  double* slots;     // [groups][slots per group][n]
+  unsigned* ticket;  // [groups], zero between launches
+};
+// host: workspace of the current device and `stream` for `n_doubles` partials and `groups`
+// tickets (thread-safe; launches on other streams use other workspaces)
+int ab_ordered_ws(cudaStream_t stream, int64_t n_doubles, int groups, Ordered* out);
+__device__ __forceinline__ double* ordered_slot(const Ordered& o, int group, int nslots, int slot,
+                                                int n) {
+  return o.slots + ((size_t)group * nslots + slot) * n;
+}
+// Called by all `nt` threads (index t) of the CTA's participating group after its partials are
+// stored; bar() synchronises that group; add(i, sum) receives the ordered total of value i.
+template <class Bar, class Add>
+__device__ __forceinline__ void ordered_finish(const Ordered& o, int group, int nslots, int n,
+                                               int t, int nt, int nctas, Bar bar, Add add,
+                                               unsigned* s_flag) {
+  __threadfence();
+  bar();
+  if (t == 0) *s_flag = atomicAdd(o.ticket + group, 1u) == (unsigned)nctas - 1u;
+  bar();
+  if (*s_flag) {
+    __threadfence();
+    const double* base = o.slots + (size_t)group * nslots * n;
+    for (int i = t; i < n; i += nt) {
+      double sum = 0.0;
+      for (int s = 0; s < nslots; ++s) sum += __ldcg(base + (size_t)s * n + i);
+      add(i, sum);
+    }
+    if (t == 0) o.ticket[group] = 0u;
+  }
+}

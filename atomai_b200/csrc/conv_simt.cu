@@ -3,7 +3,7 @@
 // input through the same normalise-on-load source loader as the tensor-core path.  This is the
 // AB_MATH_FP32 math mode: bit-for-bit it is still not the CPU reference (different summation
 // order) but it carries no TF32 rounding, so it is the mode the 1e-3 logit parity bound is pinned
-// with.  It also serves every layer shape the tcgen05 kernels do not take (C % 8 != 0, Cout % 16).
+// with.  It also serves every layer shape the tensor-core kernels do not take (C % 8 != 0, Cout % 16).
 //
 // Replaces nn.Conv2d/nn.Conv1d (+bias, LeakyReLU, BN statistics) of atomai/nets/blocks.py:61-76,
 // :302-319, :130-132 and autograd's bwd-filter for atomai/trainers/trainer.py:206.
@@ -31,6 +31,7 @@ struct ConvSimtParams {
   double* stats;
   int tiles_h, tiles_w;
   int c0;          // thin-channel kernels: first output channel of this launch's channel block
+  Ordered red;     // quad-lane / tile kernels: ordered sum of the per-warp statistics
 };
 
 __global__ void __launch_bounds__(F_THREADS) conv_simt_fwd_kernel(const ConvSimtParams p) {
@@ -163,8 +164,7 @@ __global__ void __launch_bounds__(256) conv_pix_kernel(const ConvSimtParams p, i
   // 1x1 kernel on one plain source (the pixel-wise head and its data gradient): no halo, so the
   // pending BatchNorm affine folds into the staged weights — w'[c][k] = w[c][k]*scale[c],
   // b'[k] = b[k] + sum_c w[c][k]*shift[c] — and the loop is pointer + loads + FMAs (the generic
-  // loader below re-derives source, bounds and affine for every 4 channels: ncu showed 540
-  // instructions per pixel for the 16 -> 3 head)
+  // loader below re-derives source, bounds and affine for every 4 channels)
   const bool direct = taps == 1 && p.S.nsrc == 1 && p.S.s[0].pool == 0;
   if (direct) {
     const SrcDev sd = p.S.s[0];
@@ -413,8 +413,8 @@ __global__ void __launch_bounds__(256, 2) conv_c1_kernel(const ConvSimtParams p)
 // 66 x 18 input halo tile (affine applied, zero padded) sits in shared memory; the NEXT tile's
 // halo is fetched into registers before the current one is computed.  Lane l of a warp = pixel
 // l >> 2 of an 8-pixel run x channel quad l & 3, so every STG.128 of a warp writes 8 whole pixels
-// = 512 contiguous bytes (the pair-per-thread kernel above writes 16-byte pieces 128 bytes apart:
-// 51 % excess sectors in the ncu capture), the thread's 9 x 4 weights live in registers for the
+// = 512 contiguous bytes (the pair-per-thread kernel above writes 16-byte pieces 128 bytes
+// apart), the thread's 9 x 4 weights live in registers for the
 // whole kernel, and walking down the 16 rows costs 3 broadcast LDS per 36 FFMA.  Accumulation
 // order per output (bias, then taps 0..8 with fmaf) is the pair kernel's: results are identical.
 constexpr int C1T_W = 64, C1T_H = 16, C1T_PW = C1T_W + 2, C1T_PH = C1T_H + 2;
@@ -454,7 +454,7 @@ template <int FAST>
 __global__ void __launch_bounds__(256) conv_c1_tile_kernel(const ConvSimtParams p, int tiles_w,
                                                            int tiles_hw, int num_tiles) {
   __shared__ float s_x[C1T_ELEMS];
-  __shared__ float s_red[32];
+  __shared__ unsigned s_last;
   const int c0 = p.c0;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int px = lane >> 2, q = lane & 3;
@@ -466,7 +466,6 @@ __global__ void __launch_bounds__(256) conv_c1_tile_kernel(const ConvSimtParams 
     for (int k = 0; k < 4; ++k) wr[t][k] = __ldg(p.w + (size_t)t * p.Cout + c0 + q * 4 + k);
 #pragma unroll
   for (int k = 0; k < 4; ++k) bq[k] = p.bias ? __ldg(p.bias + c0 + q * 4 + k) : 0.f;
-  if (threadIdx.x < 32) s_red[threadIdx.x] = 0.f;
   const SrcDev sd = p.S.s[0];
   float sc = 1.f, sh = 0.f;
   if (sd.scale) { sc = __ldg(sd.scale); sh = __ldg(sd.shift); }
@@ -527,16 +526,15 @@ __global__ void __launch_bounds__(256) conv_c1_tile_kernel(const ConvSimtParams 
         a += __shfl_xor_sync(0xffffffffu, a, m);
         b += __shfl_xor_sync(0xffffffffu, b, m);
       }
-      if (lane < 4) {
-        atomicAdd(&s_red[q * 4 + k], a);
-        atomicAdd(&s_red[16 + q * 4 + k], b);
+      if (lane < 4) {   // one slot per warp, added in (CTA, warp) order
+        double* slot = ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + (threadIdx.x >> 5), 32);
+        slot[q * 4 + k] = a;
+        slot[16 + q * 4 + k] = b;
       }
     }
-    __syncthreads();
-    if (threadIdx.x < 16) {
-      atomicAdd(p.stats + c0 + threadIdx.x, (double)s_red[threadIdx.x]);
-      atomicAdd(p.stats + p.Cout + c0 + threadIdx.x, (double)s_red[16 + threadIdx.x]);
-    }
+    ordered_finish(p.red, 0, gridDim.x * 8, 32, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
+                   [&](int i, double v) { p.stats[(i < 16 ? c0 : p.Cout + c0 - 16) + i] += v; },
+                   &s_last);
   }
 }
 
@@ -548,10 +546,12 @@ int launch_conv_c1_tile(const ConvSimtParams& p, cudaStream_t stream) {
   const int64_t cap = (int64_t)ab_num_sms() * 3;
   if (blocks > cap) blocks = cap;
   const bool fast = p.act == AB_ACT_LRELU && p.alpha >= 0.f && p.alpha <= 1.f;
+  ConvSimtParams q = p;
+  if (p.stats && ab_ordered_ws(stream, blocks * 8 * 32, 1, &q.red)) return 1;
   if (fast)
-    conv_c1_tile_kernel<1><<<(unsigned)blocks, 256, 0, stream>>>(p, tiles_w, tiles_w * tiles_h, (int)tiles);
+    conv_c1_tile_kernel<1><<<(unsigned)blocks, 256, 0, stream>>>(q, tiles_w, tiles_w * tiles_h, (int)tiles);
   else
-    conv_c1_tile_kernel<0><<<(unsigned)blocks, 256, 0, stream>>>(p, tiles_w, tiles_w * tiles_h, (int)tiles);
+    conv_c1_tile_kernel<0><<<(unsigned)blocks, 256, 0, stream>>>(q, tiles_w, tiles_w * tiles_h, (int)tiles);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -576,12 +576,11 @@ int launch_conv_c1(const ConvSimtParams& p, cudaStream_t stream) {
 // pieces 64 bytes apart).  Same per-output fmaf order as conv_pix_kernel's direct path.
 template <int CIN_MAX>
 __global__ void __launch_bounds__(256) conv_pix_quad_kernel(const ConvSimtParams p) {
-  __shared__ float s_red[32];
+  __shared__ unsigned s_last;
   const int lane = threadIdx.x & 31;
   const int px = lane >> 2, q = lane & 3;
   const int Cin = p.S.Ctot;
   const SrcDev sd = p.S.s[0];
-  if (threadIdx.x < 32) s_red[threadIdx.x] = 0.f;
   float wr[CIN_MAX][4], bq[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) bq[k] = p.bias ? __ldg(p.bias + q * 4 + k) : 0.f;
@@ -639,16 +638,14 @@ __global__ void __launch_bounds__(256) conv_pix_quad_kernel(const ConvSimtParams
         a += __shfl_xor_sync(0xffffffffu, a, m);
         b += __shfl_xor_sync(0xffffffffu, b, m);
       }
-      if (lane < 4) {
-        atomicAdd(&s_red[q * 4 + k], a);
-        atomicAdd(&s_red[16 + q * 4 + k], b);
+      if (lane < 4) {   // one slot per warp, added in (CTA, warp) order
+        double* slot = ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + (threadIdx.x >> 5), 32);
+        slot[q * 4 + k] = a;
+        slot[16 + q * 4 + k] = b;
       }
     }
-    __syncthreads();
-    if (threadIdx.x < 16) {
-      atomicAdd(p.stats + threadIdx.x, (double)s_red[threadIdx.x]);
-      atomicAdd(p.stats + p.Cout + threadIdx.x, (double)s_red[16 + threadIdx.x]);
-    }
+    ordered_finish(p.red, 0, gridDim.x * 8, 32, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
+                   [&](int i, double v) { p.stats[(i < 16 ? 0 : p.Cout - 16) + i] += v; }, &s_last);
   }
 }
 
@@ -663,8 +660,10 @@ int launch_conv_pix_quad(const ConvSimtParams& p, cudaStream_t stream) {
   const int64_t cap = (int64_t)ab_num_sms() * 8;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  if (p.S.Ctot <= 4) conv_pix_quad_kernel<4><<<(unsigned)blocks, 256, 0, stream>>>(p);
-  else conv_pix_quad_kernel<8><<<(unsigned)blocks, 256, 0, stream>>>(p);
+  ConvSimtParams q = p;
+  if (p.stats && ab_ordered_ws(stream, blocks * 8 * 32, 1, &q.red)) return 1;
+  if (p.S.Ctot <= 4) conv_pix_quad_kernel<4><<<(unsigned)blocks, 256, 0, stream>>>(q);
+  else conv_pix_quad_kernel<8><<<(unsigned)blocks, 256, 0, stream>>>(q);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -703,6 +702,7 @@ struct WgradSimtParams {
   int64_t npix;
   int px_per_cta;
   int co_tiles, ci_tiles;
+  Ordered red;     // quad-lane / tile kernels: ordered sum of the per-warp partial dW
 };
 
 __global__ void __launch_bounds__(G_THREADS) conv_simt_wgrad_kernel(const WgradSimtParams p) {
@@ -846,11 +846,9 @@ __global__ void __launch_bounds__(256, 2) wgrad_c1_kernel(const WgradSimtParams 
 __global__ void __launch_bounds__(256) wgrad_c1_tile_kernel(const WgradSimtParams p, int tiles_w,
                                                             int tiles_hw, int num_tiles) {
   __shared__ float s_x[C1T_ELEMS];
-  __shared__ float s_acc[16 * 9];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int px = lane >> 2, q = lane & 3;
   const int col = warp * 8 + px;
-  for (int i = threadIdx.x; i < 16 * 9; i += blockDim.x) s_acc[i] = 0.f;
   const SrcDev sd = p.S.s[0];
   float sc = 1.f, sh = 0.f;
   if (sd.scale) { sc = __ldg(sd.scale); sh = __ldg(sd.shift); }
@@ -911,10 +909,12 @@ __global__ void __launch_bounds__(256) wgrad_c1_tile_kernel(const WgradSimtParam
       float v = acc[k][t];
 #pragma unroll
       for (int m = 4; m <= 16; m <<= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
-      if (lane < 4) atomicAdd(&s_acc[(q * 4 + k) * 9 + t], v);
+      if (lane < 4)     // one slot per warp, added in (CTA, warp) order
+        ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + warp, 16 * 9)[(q * 4 + k) * 9 + t] = v;
     }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 16 * 9; i += blockDim.x) atomicAdd(p.dw + i, s_acc[i]);   // OIHW, Cin = 1
+  __shared__ unsigned s_last;
+  ordered_finish(p.red, 0, gridDim.x * 8, 16 * 9, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
+                 [&](int i, double v) { p.dw[i] += (float)v; }, &s_last);   // OIHW, Cin = 1
 }
 
 int launch_wgrad_c1_tile(const WgradSimtParams& p, cudaStream_t stream) {
@@ -924,7 +924,9 @@ int launch_wgrad_c1_tile(const WgradSimtParams& p, cudaStream_t stream) {
   int64_t blocks = tiles;
   const int64_t cap = (int64_t)ab_num_sms() * 3;
   if (blocks > cap) blocks = cap;
-  wgrad_c1_tile_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p, tiles_w, tiles_w * tiles_h, (int)tiles);
+  WgradSimtParams q = p;
+  if (ab_ordered_ws(stream, blocks * 8 * 16 * 9, 1, &q.red)) return 1;
+  wgrad_c1_tile_kernel<<<(unsigned)blocks, 256, 0, stream>>>(q, tiles_w, tiles_w * tiles_h, (int)tiles);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -1040,12 +1042,10 @@ __global__ void __launch_bounds__(256) wgrad_small_kernel(const WgradSimtParams 
 // read with 512-byte coalesced LDG.128 rows (thread-per-pixel: four 16-byte pieces 64 bytes
 // apart per thread); the <= 4 dy values of a pixel are one broadcast request per quad.
 __global__ void __launch_bounds__(256) wgrad_pix_quad_kernel(const WgradSimtParams p) {
-  __shared__ float s_acc[4 * 16];
   const int lane = threadIdx.x & 31;
   const int q = lane & 3;
   const int Cout = p.Cout;
   const SrcDev sd = p.S.s[0];
-  if (threadIdx.x < 64) s_acc[threadIdx.x] = 0.f;
   float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
   if (sd.scale) {
     sc = __ldg(reinterpret_cast<const float4*>(sd.scale + q * 4));
@@ -1078,11 +1078,13 @@ __global__ void __launch_bounds__(256) wgrad_pix_quad_kernel(const WgradSimtPara
       float v = acc[a][b];
 #pragma unroll
       for (int m = 4; m <= 16; m <<= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
-      if (lane < 4) atomicAdd(&s_acc[a * 16 + q * 4 + b], v);
+      if (lane < 4)     // one slot per warp, added in (CTA, warp) order
+        ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + (threadIdx.x >> 5), 64)[a * 16 + q * 4 + b] = v;
     }
-  __syncthreads();
-  if (threadIdx.x < 64 && (threadIdx.x >> 4) < Cout)                // OIHW with 1x1 taps
-    atomicAdd(p.dw + (size_t)(threadIdx.x >> 4) * 16 + (threadIdx.x & 15), s_acc[threadIdx.x]);
+  __shared__ unsigned s_last;
+  ordered_finish(p.red, 0, gridDim.x * 8, 64, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
+                 [&](int i, double v) { if ((i >> 4) < Cout) p.dw[(size_t)(i >> 4) * 16 + (i & 15)] += (float)v; },
+                 &s_last);                                            // OIHW with 1x1 taps
 }
 
 int launch_wgrad_pix_quad(const WgradSimtParams& p, cudaStream_t stream) {
@@ -1090,7 +1092,9 @@ int launch_wgrad_pix_quad(const WgradSimtParams& p, cudaStream_t stream) {
   const int64_t cap = (int64_t)ab_num_sms() * 8;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  wgrad_pix_quad_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p);
+  WgradSimtParams q = p;
+  if (ab_ordered_ws(stream, blocks * 8 * 64, 1, &q.red)) return 1;
+  wgrad_pix_quad_kernel<<<(unsigned)blocks, 256, 0, stream>>>(q);
   AB_LAUNCH_CHECK();
   return 0;
 }

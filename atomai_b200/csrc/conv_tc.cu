@@ -1,19 +1,22 @@
-// conv_tc.cu — implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05, TF32 operands,
-// fp32 accumulators in TMEM).  One persistent, warp-specialised CTA per SM:
+// conv_tc.cu — implicit-GEMM convolution on the Hopper tensor cores (wgmma, TF32 operands, fp32
+// accumulators in registers).  One persistent, warp-specialised CTA per SM:
 //
-//   warps 0-3   epilogue   TMEM -> regs -> bias + LeakyReLU -> NHWC/NCHW store + BN statistics
-//   warp  4     MMA issue  one elected lane issues tcgen05.mma for every (k-chunk, tap, k-step)
-//   warp  5     weights    TMEM alloc + cp.async.bulk of pre-packed weight blobs (L2 -> smem)
+//   warps 0-3   consumer   wgmma for every (k-chunk, tap, k-step) of a tile, then the epilogue from
+//                          the accumulator registers: bias + activation -> NHWC/NCHW store + BN statistics
+//   warps 5, 7  producers  cp.async.bulk of pre-packed weight blobs (L2 -> smem), TMA activation tiles
 //   warps 8-15  loaders    HBM/L2 -> regs -> [BN affine, 2x2 max-pool, zero pad, RN->TF32] -> smem
-//                          (two groups of 4 warps working on alternate k-chunks; setmaxnreg moves
-//                          registers from the MMA/epilogue warpgroups to the loaders)
+//                          (two groups of 4 warps = two pipelines working on alternate tiles;
+//                          setmaxnreg moves registers from the producer warpgroup to the others)
 //
-// GEMM view (SURVEY.md §8a): M = 128 output pixels (a 16 x 8 tile), N = Cout, K = taps * Cin.
-// The activation halo tile is loaded ONCE per 32-channel chunk and re-used by all nine taps: it
-// is stored as UMMA "interleave" (no-swizzle) K-major core matrices, one plane per 4 channels,
-// rows = halo pixels at 16 B pitch.  A tap is then just a different start address
-// ((ty*d*TWp + tx*d) * 16 B) with SBO = TWp*16 B (next image row = next 8-row group) and
-// LBO = plane stride (next 4 channels).  No im2col buffer ever exists.
+// GEMM view (SURVEY.md §8a): M = 64 output pixels (an 8 x 8 tile = one m64 wgmma row block, or
+// 8 x 16 as two sub-tiles when N <= 64), N = Cout (<= 128 per launch; wider layers run one launch
+// per 128 channels), K = taps * Cin.  The tile height is set by the register file: the whole
+// 512-thread kernel is compiled for 128 registers per thread, so the consumer keeps at most 64
+// fp32 accumulators.  The activation halo tile is loaded ONCE per k-chunk and re-used by all nine
+// taps: it is stored as K-major no-swizzle core matrices, one plane per 4 channels, rows = halo
+// pixels at 16 B pitch.  A tap is then just a different start address ((ty*d*TWp + tx*d) * 16 B)
+// with SBO = TWp*16 B (next image row = next 8-row group) and LBO = plane stride (next 4
+// channels).  No im2col buffer ever exists.
 //
 // Replaces nn.Conv2d(+bias) -> nn.LeakyReLU -> (batch statistics of) nn.BatchNorm2d of
 // atomai/nets/blocks.py:61-76,302-319, the preceding BatchNorm2d/max_pool2d/cat passes
@@ -23,29 +26,26 @@
 #include <cstdio>
 #include <cstdlib>
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int kTileH = 16;
+constexpr int kTileH = 8;
 constexpr int kTileW = 8;
-constexpr int kNumEpiWarps = 4;     // per epilogue group (one warp per TMEM lane quadrant)
-constexpr int kEpiGroups = 1;       // 2: group e drains the accumulators of pipeline e (warps 0-3, 16-19)
-constexpr int kEpiBWarp = 16;       // first warp of epilogue group 1
-constexpr int kMmaWarp = 4;
+constexpr int kNumEpiWarps = 4;     // the consumer warpgroup
 constexpr int kWgtWarp = 5;
-constexpr int kMmaWarp2 = 6;          // second issuing thread
-constexpr int kWgtWarp2 = 7;          // second weight producer (streamed weights)
-constexpr int kFirstLoadWarp = 8;   // warps 6,7 idle: roles are aligned to 4-warp groups (setmaxnreg)
+constexpr int kWgtWarp2 = 7;        // second weight / TMA producer (pipeline 1)
+constexpr int kFirstLoadWarp = 8;
 constexpr int kNumLoadWarps = 8;
-constexpr int kThreads = (kFirstLoadWarp + kNumLoadWarps + (kEpiGroups - 1) * kNumEpiWarps) * 32;
-// register re-balancing between the warpgroups (sum * 128 threads = 64K registers).  A second
-// epilogue group (kEpiGroups = 2, 640 threads) was tried in round 2 — the ncu source view shows
-// the epilogue warps never waiting while loaders and the MMA thread do — but ptxas allocates for
-// the launch bound (96 registers at 640 threads) whatever setmaxnreg says, and the spills cost
-// more than the second group gains.
-constexpr int kRegsEpi = kEpiGroups == 1 ? 112 : 128, kRegsMma = kEpiGroups == 1 ? 72 : 48,
-              kRegsLoad = kEpiGroups == 1 ? 160 : 104;
-static_assert(kEpiGroups * kRegsEpi + kRegsMma + 2 * kRegsLoad <= 512, "register budget");
+constexpr int kThreads = (kFirstLoadWarp + kNumLoadWarps) * 32;
+constexpr int kEpiBWarp = kThreads / 32;
+// register re-balancing between the warpgroups (sum * 128 threads = 64K registers).  ptxas still
+// allocates every branch for the 512-thread launch bound (128 registers per thread), so these
+// values only move the physical registers; the consumer's SUB * N / 2 <= 64 fp32 accumulators are
+// what fits that bound (the epilogue spills some of its temporaries to the stack)
+constexpr int kRegsEpi = 232, kRegsMma = 40, kRegsLoad = 120;
+static_assert(kRegsEpi + kRegsMma + 2 * kRegsLoad <= 512, "register budget");
+constexpr int kMaxN = 128;          // output channels per launch (accumulator registers)
 constexpr int kMaxAStages = 4;
 constexpr int kMaxBStages = 32;     // streamed weights: bytes in flight must cover the L2 latency
 constexpr int kMaxRStages = 8;      // TMA mode: raw activation tiles in flight (two rings of n_r/2)
@@ -55,6 +55,7 @@ constexpr int kMaxU = 12;           // register-staged 16B elements per loader t
 struct ConvTcParams {
   SrcSet S;
   int N, H, W, Cout;
+  int n0, nn;        // output channels [n0, n0 + nn) of this launch
   int taps_h, taps_w, dil;
   const float* wblob;
   const float* bias;
@@ -65,6 +66,7 @@ struct ConvTcParams {
   int out_nchw;
   int64_t nchw_stride; // out_nchw: elements between channel planes (H*W, or the caller's row pitch)
   double* stats;
+  Ordered red;       // stats: ordered sum of the per-CTA partials
   int tiles_h, tiles_w, num_tiles;
   int KC;            // channels per k-chunk (8, 16 or 32)
   int n_chunks;      // Ctot / KC
@@ -72,136 +74,235 @@ struct ConvTcParams {
   int plane_bytes;   // stride between 4-channel planes (== 128/P mod 128 -> conflict-free STS)
   int a_stage_bytes, b_stage_bytes;
   int n_a, n_b;      // pipeline depths
-  int n_acc;         // TMEM accumulator buffers: 4 (two per pipeline) or 2 (one per pipeline)
-  int tmem_cols;     // power of two >= n_acc*sub*Cout
   int sub;           // 8-pixel-wide sub-tiles per CTA tile (1 or 2): M = 128*sub per weight stage
   int w_resident;    // 1: all weights live in shared memory for the whole kernel
   int w_bytes;       // taps * Ctot * Cout * 4  (x3: twice that — hi and lo parts)
-  int x3;            // AB_MATH_TF32X3: every k-step issues a second, kind::f16 MMA on a bf16 operand
+  int x3;            // AB_MATH_TF32X3: every k-step issues a second, bf16 MMA (K = 16) on an operand
                      // pair ([a_lo | a_hi] x [w ; w_lo]) that adds the two cross terms of the split
   int corr_off;      // x3: byte offset of the correction planes inside an activation stage
   // TMA mode (resident weights, un-pooled sources): cp.async.bulk.tensor copies the raw NHWC halo
   // tile {KC channels, TWp, THp} (out-of-image pixels zero-filled by the copy engine) into a ring
   // of raw stages; the "loader" warps then only transform shared memory -> shared memory (affine,
-  // border mask, TF32 rounding / x3 split into the UMMA planes).  Bytes in flight are bounded by
+  // border mask, TF32 rounding / x3 split into the MMA planes).  Bytes in flight are bounded by
   // the raw ring (up to 8 stages) instead of by loader registers.
   int tma;
   int raw_bytes;     // HP * KC * 4
   int n_r;           // raw stages (two rings of n_r/2)
-  int dbg;           // bring-up only (ATOMAI_B200_DBG): bit 0 skip the global stores, bit 1 skip the TMEM loads
 };
 
 struct __align__(8) SharedCtl {
   uint64_t full_a[kMaxAStages], empty_a[kMaxAStages];
   uint64_t full_b[kMaxBStages], empty_b[kMaxBStages];
-  uint64_t tmem_full[4], tmem_empty[4];
   uint64_t raw_full[kMaxRStages], raw_empty[kMaxRStages];
   uint64_t w_full;
-  uint32_t tmem_base;
-  uint32_t pad;
+  unsigned red_last;
 };
 
-
-// The MMA-issuing thread's whole tile loop, specialised on (k-steps per chunk, sub-tiles,
-// resident weights) so that the per-MMA work is two 32-bit adds + the tcgen05.mma.
-template <int KSTEPS, int SUB, bool RESIDENT>
-__device__ __forceinline__ void mma_issue_loop(const ConvTcParams& p, SharedCtl* ctl,
-                                               uint32_t tmem_base, uint32_t a_base,
-                                               uint32_t b_base, int issuer) {
-  const uint32_t idesc = umma_idesc_tf32(128, p.Cout, 0, 0);
-  const uint32_t piece16 = (uint32_t)p.Cout * 32 >> 4;
-  const uint64_t a_tmpl = umma_desc(0, p.plane_bytes, p.TWp * 16);
-  const uint64_t b_tmpl = umma_desc(0, p.Cout * 16, 128);
-  const uint32_t a_hi = (uint32_t)(a_tmpl >> 32), b_hi = (uint32_t)(b_tmpl >> 32);
-  const uint32_t a_lo0 = (uint32_t)a_tmpl + (a_base >> 4), b_lo0 = (uint32_t)b_tmpl + (b_base >> 4);
-  const uint32_t n_a = p.n_a, n_b = p.n_b, n_chunks = p.n_chunks, cout = p.Cout;
-  const uint32_t a_stage16 = p.a_stage_bytes >> 4, b_stage16 = p.b_stage_bytes >> 4;
-  const uint32_t plane2_16 = (uint32_t)p.plane_bytes * 2 >> 4;     // next k-step of A
-  const uint32_t dx16 = p.dil, dy16 = (uint32_t)p.dil * p.TWp;     // tap steps of A (16 B units)
-  const int th = p.taps_h, tw = p.taps_w, taps = th * tw;
-  // resident weights: piece index = (chunk*KSTEPS + ks)*taps + t
-  // (x3: the blob interleaves a main and a correction piece per k-step, see
-  //  pack_weights_tc_kernel; a streamed weight stage holds [k-step][main, corr] pieces)
-  const bool x3 = p.x3 != 0;
-  const uint32_t wmult = x3 ? 2u : 1u;
-  const uint32_t b_ks16 = RESIDENT ? wmult * (uint32_t)taps * piece16 : wmult * piece16;
-  const uint32_t chunk_w16 = wmult * (uint32_t)(KSTEPS * taps) * piece16;
-  const uint32_t corr_w16 = RESIDENT ? (uint32_t)taps * piece16 : piece16;   // main -> corr piece
-  const uint32_t corr_a16 = (uint32_t)p.corr_off >> 4;                       // main -> corr planes
-  const uint32_t idesc_c = umma_idesc_bf16(128, p.Cout, 0, 0);
-  uint32_t sa = 0, pa = 0, sb = 0, pb = 0;
-  const uint32_t bar_full_a = smem_u32(&ctl->full_a[0]), bar_empty_a = smem_u32(&ctl->empty_a[0]);
-  const uint32_t bar_full_b = smem_u32(&ctl->full_b[0]), bar_empty_b = smem_u32(&ctl->empty_b[0]);
-  const uint32_t bar_tfull = smem_u32(&ctl->tmem_full[0]), bar_tempty = smem_u32(&ctl->tmem_empty[0]);
-  if (RESIDENT) {
-    mbar_wait(smem_u32(&ctl->w_full), 0);
-    tc_fence_after();
-  }
-  // Two independent pipelines per CTA: loader group i -> issuing thread i -> TMEM accumulators
-  // {i, i+2}, on the CTA's tiles with local index = i (mod 2), each with its own half of the
-  // activation-stage ring and (streamed weights) its own weight ring fed by its own producer
-  // thread.  One issuing thread costs ~150 clocks per MMA in the streamed loop (barrier wait,
-  // descriptor moves, commit) against 40-64 clocks of tensor-pipe time, so a single issuer left
-  // the pipe two-thirds idle.  A stage barrier must have ONE consumer: with a shared ring a fast
-  // consumer aliases the parity of a phase the other one has not seen yet.
-  const uint32_t n_iss = 2u;
-  const uint32_t n_acc = p.n_acc;
-  uint32_t tl = issuer;                                  // this issuer's running local tile index
-  const uint32_t ring_n = n_a / 2;
-  const uint32_t ring0 = issuer * ring_n;
-  const uint32_t nb2 = n_b / 2;                          // weight stages of this pipeline's ring
-  const uint32_t b_ring0 = issuer * nb2;
-  const int num_tiles = p.num_tiles;
-  const int tile_step = gridDim.x * n_iss;
-  for (int tile = blockIdx.x + issuer * gridDim.x; tile < num_tiles; tile += tile_step) {
-    const uint32_t a_ = tl & (n_acc - 1);
-    mbar_wait(bar_tempty + a_ * 8, ((tl / n_acc) & 1) ^ 1);
-    tc_fence_after();
-    const uint32_t d_tmem = tmem_base + a_ * SUB * cout;
-    uint32_t accum = 0u;
-    uint32_t b_tap = b_lo0;                                        // resident: running piece
-    for (uint32_t ch = 0; ch < n_chunks; ++ch) {
-      mbar_wait(bar_full_a + (ring0 + sa) * 8, pa);
-      tc_fence_after();
-      uint32_t a_row = a_lo0 + (ring0 + sa) * a_stage16;
-      if (RESIDENT) b_tap = b_lo0 + ch * chunk_w16;
-      for (int ty = 0; ty < th; ++ty, a_row += dy16) {
-        uint32_t a_tap = a_row;
-        for (int tx = 0; tx < tw; ++tx, a_tap += dx16, b_tap += piece16) {
-          uint32_t bd = b_tap;
-          if (!RESIDENT) {
-            mbar_wait(bar_full_b + (b_ring0 + sb) * 8, pb);
-            tc_fence_after();
-            bd = b_lo0 + (b_ring0 + sb) * b_stage16;
-          }
-          uint32_t ad = a_tap;
-#pragma unroll
-          for (int ks = 0; ks < KSTEPS; ++ks, ad += plane2_16, bd += b_ks16) {
-            umma_tf32_lh(d_tmem, ad, a_hi, bd, b_hi, idesc, accum);
-            if (SUB > 1) umma_tf32_lh(d_tmem + cout, ad + (kTileW * 16 >> 4), a_hi, bd, b_hi, idesc, accum);
-            accum = 1u;
-            if (x3) {   // + a_lo*w + a_hi*w_lo: one bf16 MMA (K = 16) on the correction planes
-              umma_bf16_lh(d_tmem, ad + corr_a16, a_hi, bd + corr_w16, b_hi, idesc_c, 1u);
-              if (SUB > 1)
-                umma_bf16_lh(d_tmem + cout, ad + corr_a16 + (kTileW * 16 >> 4), a_hi, bd + corr_w16,
-                             b_hi, idesc_c, 1u);
-            }
-          }
-          if (!RESIDENT) {
-            umma_commit(bar_empty_b + (b_ring0 + sb) * 8);
-            if (++sb == nb2) { sb = 0; pb ^= 1; }
-          }
-        }
-      }
-      umma_commit(bar_empty_a + (ring0 + sa) * 8);
-      if (++sa == ring_n) { sa = 0; pa ^= 1; }
-    }
-    umma_commit(bar_tfull + a_ * 8);
-    tl += n_iss;
+// consumer warp: every warp of the group arrives once it has seen its MMAs retire
+__device__ __forceinline__ void consumer_release(uint32_t bar) {
+  if (bar) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
   }
 }
 
-// RN-to-TF32 of an fp32 bit pattern for a tcgen05 operand: the tensor core reads only the upper
+// The consumer warpgroup's whole tile loop, specialised on (N = output channels of this launch,
+// 8-pixel sub-tiles).  Tiles alternate between the two pipelines (loader group / weight ring i
+// stages the tiles with local index = i mod 2).  A k-chunk (resident weights) or a tap (streamed
+// weights) is one wgmma group; a stage is handed back to its producer when the group after its
+// last use has been issued and the one using it has retired (wgmma.wait_group 1), so the tensor
+// core always has the next group queued.
+template <int N, int SUB>
+__device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* ctl, uint32_t a_base,
+                                              uint32_t b_base, float* s_stats, const float* s_bias) {
+  constexpr int R = N / 2;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t ring_n = p.n_a / 2, nb2 = p.n_b / 2;
+  const int ksteps = p.KC >> 3;
+  const int th = p.taps_h, tw = p.taps_w, taps = th * tw;
+  const bool x3 = p.x3 != 0, res = p.w_resident != 0;
+  const uint32_t wmult = x3 ? 2u : 1u;
+  const uint32_t piece = (uint32_t)p.Cout * 32;                     // bytes of one (k-step, tap) piece
+  const uint32_t corr_w = res ? (uint32_t)taps * piece : piece;      // main -> correction piece
+  const uint32_t b_n0 = (uint32_t)p.n0 * 16;
+  const uint64_t a_tmpl = wgmma_desc(0, p.plane_bytes, p.TWp * 16);
+  const uint64_t b_tmpl = wgmma_desc(0, p.Cout * 16, 128);
+  const uint32_t mb_off = 8u * p.TWp * 16, sb_off = kTileW * 16;
+  const uint32_t bar_full_a = smem_u32(&ctl->full_a[0]), bar_empty_a = smem_u32(&ctl->empty_a[0]);
+  const uint32_t bar_full_b = smem_u32(&ctl->full_b[0]), bar_empty_b = smem_u32(&ctl->empty_b[0]);
+  const int tpi = p.tiles_w * p.tiles_h;
+  const bool fast = p.act == AB_ACT_LRELU && p.alpha >= 0.f && p.alpha <= 1.f;
+  const float alpha = p.alpha;
+  float* my_stats = s_stats + warp * 2 * p.Cout;
+  if (res) mbar_wait_quiet(smem_u32(&ctl->w_full), 0);
+  uint32_t sa0 = 0, pa0 = 0, sb0 = 0, pb0 = 0, sa1 = 0, pa1 = 0, sb1 = 0, pb1 = 0;
+  constexpr int MB = kTileH / 8;               // m64 row blocks per sub-tile
+  float acc[SUB][MB][R];
+
+  auto tile_fn = [&](const int tile, const int pipe, uint32_t& s_a, uint32_t& p_a, uint32_t& s_b,
+                     uint32_t& p_b) {
+    const uint32_t ring0 = pipe * ring_n, b_ring0 = pipe * nb2;
+    uint32_t pend_a = 0, pend_b = 0, accum = 0;
+    for (int ch = 0; ch < p.n_chunks; ++ch) {
+      if (pend_a && ring_n == 1) {
+        // one operand stage per pipeline: the stage this chunk needs is the one still held for
+        // the previous chunk, so its MMAs must retire before it can go back to the loaders
+        wgmma_wait<0>();
+        consumer_release(pend_a);
+        pend_a = 0;
+      }
+      mbar_wait_quiet(bar_full_a + (ring0 + s_a) * 8, p_a);
+      const uint32_t a_stage = a_base + (ring0 + s_a) * p.a_stage_bytes;
+      for (int t = 0; t < taps; ++t) {
+        const int ty = t / tw, tx = t - ty * tw;
+        uint32_t b_stage = 0;
+        if (!res) {
+          if (pend_b && nb2 == 1) {   // the same for a one-stage weight ring
+            wgmma_wait<0>();
+            consumer_release(pend_b);
+            pend_b = 0;
+          }
+          mbar_wait_quiet(bar_full_b + (b_ring0 + s_b) * 8, p_b);
+          b_stage = b_base + (b_ring0 + s_b) * p.b_stage_bytes;
+        }
+        const uint32_t a_tap = a_stage + (uint32_t)(ty * p.TWp + tx) * p.dil * 16;
+        wgmma_fence();
+        for (int ks = 0; ks < ksteps; ++ks) {
+          const uint32_t a_k = a_tap + ks * 2u * p.plane_bytes;
+          const uint32_t b_k = b_n0 + (res ? b_base + ((uint32_t)(ch * ksteps + ks) * wmult * taps + t) * piece
+                                           : b_stage + ks * wmult * piece);
+          const uint64_t bd = b_tmpl | (b_k >> 4);
+#pragma unroll
+          for (int s = 0; s < SUB; ++s)
+#pragma unroll
+            for (int mb = 0; mb < MB; ++mb)
+              Wgmma<N>::tf32(acc[s][mb], a_tmpl | ((a_k + mb * mb_off + s * sb_off) >> 4), bd, accum);
+          if (x3) {   // + a_lo*w + a_hi*w_lo: one bf16 MMA (K = 16) on the correction planes
+            const uint64_t bc = b_tmpl | ((b_k + corr_w) >> 4);
+#pragma unroll
+            for (int s = 0; s < SUB; ++s)
+#pragma unroll
+              for (int mb = 0; mb < MB; ++mb)
+                Wgmma<N>::bf16(acc[s][mb], a_tmpl | ((a_k + p.corr_off + mb * mb_off + s * sb_off) >> 4),
+                               bc, 1u);
+          }
+          accum = 1u;
+        }
+        // resident weights: one group per k-chunk; streamed: one per tap (its weight stage goes
+        // back as soon as possible, the ring may hold fewer stages than there are taps)
+        if (res && t != taps - 1) continue;
+        wgmma_commit();
+        wgmma_wait<1>();
+        consumer_release(pend_a);
+        consumer_release(pend_b);
+        pend_a = 0;
+        pend_b = 0;
+        if (!res) {
+          pend_b = bar_empty_b + (b_ring0 + s_b) * 8;
+          if (++s_b == nb2) { s_b = 0; p_b ^= 1; }
+        }
+        if (t == taps - 1) {
+          pend_a = bar_empty_a + (ring0 + s_a) * 8;
+          if (++s_a == ring_n) { s_a = 0; p_a ^= 1; }
+        }
+      }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int s = 0; s < SUB; ++s)
+#pragma unroll
+      for (int mb = 0; mb < MB; ++mb) wgmma_fence_regs(acc[s][mb]);
+    consumer_release(pend_a);
+    consumer_release(pend_b);
+
+    // ---------------- epilogue: registers -> bias + activation -> global store + BN statistics
+    const int n = tile / tpi, rem = tile - n * tpi;
+    const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
+    const int c_lane = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < R / 4; ++j) {
+      const int cl = 8 * j + c_lane;              // column within this launch
+      const int c = p.n0 + cl;
+      const float b0 = s_bias[c], b1 = s_bias[c + 1];
+      float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+      for (int s = 0; s < SUB; ++s)
+#pragma unroll
+        for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+          for (int hrow = 0; hrow < 2; ++hrow) {
+            const int gh = th_i * kTileH + mb * 8 + 2 * warp + hrow;
+            const int gw = (tw_i * SUB + s) * kTileW + (lane >> 2);
+            const bool valid = gh < p.H && gw < p.W;
+            float v0 = acc[s][mb][4 * j + 2 * hrow] + b0, v1 = acc[s][mb][4 * j + 2 * hrow + 1] + b1;
+            if (fast) {
+              v0 = fmaxf(v0, v0 * alpha);
+              v1 = fmaxf(v1, v1 * alpha);
+            } else if (p.act == AB_ACT_RBF) {     // alpha * exp(-x/2) as one FMUL + EX2
+              v0 = alpha * exp2f(-0.72134752f * fmaxf(v0, 0.f));
+              v1 = alpha * exp2f(-0.72134752f * fmaxf(v1, 0.f));
+            } else {
+              v0 = act_f(v0, p.act, alpha);
+              v1 = act_f(v1, p.act, alpha);
+            }
+            v0 = valid ? v0 : 0.f;
+            v1 = valid ? v1 : 0.f;
+            if (valid) {
+              const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
+              if (!p.out_nchw) {
+                *reinterpret_cast<float2*>(p.out + pix * p.ld_out + c) = make_float2(v0, v1);
+              } else {
+                const size_t hw = (size_t)p.nchw_stride;
+                float* o = p.out + ((size_t)n * p.Cout + c) * hw + (size_t)gh * p.W + gw;
+                o[0] = v0;
+                o[hw] = v1;
+              }
+            }
+            s0 += v0; s1 += v1;
+            q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
+          }
+      if (p.stats) {   // the 8 lanes sharing (lane & 3) hold the same two channels
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {
+          s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+          s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+          q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+          q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+        }
+        if (lane < 4) {
+          my_stats[c] += s0;
+          my_stats[c + 1] += s1;
+          my_stats[p.Cout + c] += q0;
+          my_stats[p.Cout + c + 1] += q1;
+        }
+      }
+    }
+  };
+
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += 2 * gridDim.x) {
+    tile_fn(tile, 0, sa0, pa0, sb0, pb0);
+    if (tile + (int)gridDim.x < p.num_tiles) tile_fn(tile + gridDim.x, 1, sa1, pa1, sb1, pb1);
+  }
+  if (p.stats) {   // this CTA's partial = the four warps' sums in warp order, then ordered over CTAs
+    auto bar = [] { asm volatile("bar.sync 1, %0;" ::"n"(kNumEpiWarps * 32) : "memory"); };
+    bar();
+    const int t = threadIdx.x, n = 2 * p.nn;
+    double* slot = ordered_slot(p.red, 0, gridDim.x, blockIdx.x, n);
+    for (int i = t; i < n; i += kNumEpiWarps * 32) {
+      const int c = i < p.nn ? p.n0 + i : p.Cout + p.n0 + (i - p.nn);
+      double v = 0.0;
+      for (int w = 0; w < kNumEpiWarps; ++w) v += (double)s_stats[w * 2 * p.Cout + c];
+      slot[i] = v;
+    }
+    ordered_finish(p.red, 0, gridDim.x, n, t, kNumEpiWarps * 32, gridDim.x, bar,
+                   [&](int i, double v) {
+                     p.stats[i < p.nn ? p.n0 + i : p.Cout + p.n0 + (i - p.nn)] += v;
+                   },
+                   &ctl->red_last);
+  }
+}
+
+// RN-to-TF32 of an fp32 bit pattern for a tensor-core operand: the tensor core reads only the upper
 // 19 bits, so adding half an ulp of the 10-bit mantissa (round-half-away, like cvt.rna) is enough
 // and costs one integer add instead of cvt.rna.tf32's four-instruction emulation.
 __device__ __forceinline__ uint32_t tf32_bits(float x) { return __float_as_uint(x) + 0x1000u; }
@@ -312,7 +413,7 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
     if (p.tma) {
       // the copy engine has staged the raw tile (zero-filled outside the image): registers <-
       // shared memory, then hand the raw stage straight back to the producer
-      mbar_wait(bar_raw_full + (rr0 + rst) * 8, rph);
+      mbar_wait_quiet(bar_raw_full + (rr0 + rst) * 8, rph);
       const uint32_t rsrc = raw_src0 + (rr0 + rst) * p.raw_bytes;
 #pragma unroll
       for (int u = 0; u < U; ++u)
@@ -409,7 +510,7 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
         v[u] = make_float4(ok ? mx : 0.f, ok ? my : 0.f, ok ? mz : 0.f, ok ? mw : 0.f);
       }
     }
-    mbar_wait(bar_empty_a + (ring0 + st) * 8, ph);
+    mbar_wait_quiet(bar_empty_a + (ring0 + st) * 8, ph);
     const uint32_t dst = dst0 + (ring0 + st) * p.a_stage_bytes;
     if (x3) {
       const uint32_t cdst = corr_dst0 + (ring0 + st) * p.a_stage_bytes;
@@ -455,149 +556,6 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
   }
 }
 
-// Transposing butterfly: 32 per-thread values -> lane l holds the warp total of value l
-// (31 shuffles instead of 32 x 5).
-__device__ __forceinline__ float warp_transpose_sum32(float (&w)[32], int lane) {
-#pragma unroll
-  for (int sft = 16; sft >= 1; sft >>= 1) {
-    const bool up = (lane & sft) != 0;
-#pragma unroll
-    for (int k = 0; k < sft; ++k) {
-      const float send = up ? w[k] : w[k + sft];
-      const float keep = up ? w[k + sft] : w[k];
-      w[k] = keep + __shfl_xor_sync(0xffffffffu, send, sft);
-    }
-  }
-  return w[0];
-}
-
-// Epilogue warps 0-3: TMEM -> registers -> bias + activation -> global store + BN statistics.
-// NG > 0 (Cout = 16*NG <= 32, the HBM-bound thin layers): per-thread running sums live in
-// registers for the whole kernel (2 instructions per value) and are reduced once at the end;
-// NG == 0: per-tile transposing butterfly into per-warp shared-memory partials.
-// FAST 1: LeakyReLU with 0 <= slope <= 1 as max(x, slope*x); FAST 2: the Gram kernel's RBF
-// epilogue alpha * exp(-x/2) as one FMUL + EX2 (the epilogue, not the MMA, bounds that kernel).
-template <int NG, int FAST>
-__device__ __forceinline__ void epilogue_loop(const ConvTcParams& p, SharedCtl* ctl,
-                                              uint32_t tmem_base, float* s_stats,
-                                              const float* s_bias, int eg) {
-  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;   // warp within the group
-  const uint32_t n_acc = p.n_acc;
-  uint32_t tl = eg;                  // this group's local tile counter (= the issuing thread's)
-  float* my_stats = s_stats + (eg * kNumEpiWarps + warp) * 2 * p.Cout;
-  const int row = warp * 32 + lane;
-  const int r_h = row >> 3, r_w = row & 7;
-  const int tpi = p.tiles_w * p.tiles_h;
-  const float inv_tpi = 1.f / (float)tpi, inv_tw = 1.f / (float)p.tiles_w;
-  const float alpha = p.alpha;
-  constexpr int NA = NG > 0 ? NG * 16 : 16;
-  float rs[NA], rq[NA];
-#pragma unroll
-  for (int i = 0; i < NA; ++i) rs[i] = rq[i] = 0.f;
-  const bool do_stats = p.stats != nullptr;
-  for (int tile = blockIdx.x + eg * gridDim.x; tile < p.num_tiles; tile += kEpiGroups * gridDim.x) {
-    int n = __float2int_rz((float)tile * inv_tpi);
-    n += ((n + 1) * tpi <= tile) - (n * tpi > tile);
-    const int rem = tile - n * tpi;
-    int th_i = __float2int_rz((float)rem * inv_tw);
-    th_i += ((th_i + 1) * p.tiles_w <= rem) - (th_i * p.tiles_w > rem);
-    const int tw_i = rem - th_i * p.tiles_w;
-    const uint32_t acc = tl & (n_acc - 1);
-    mbar_wait(smem_u32(&ctl->tmem_full[acc]), (tl / n_acc) & 1);
-    tc_fence_after();
-    for (int sb_ = 0; sb_ < p.sub; ++sb_) {
-      const int gh = th_i * kTileH + r_h, gw = (tw_i * p.sub + sb_) * kTileW + r_w;
-      const bool valid = gh < p.H && gw < p.W;
-      const uint32_t t_addr =
-          tmem_base + (acc * p.sub + sb_) * p.Cout + ((uint32_t)(warp * 32) << 16);
-      const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
-      auto group = [&](const int g, const int gi) {
-        const int c0 = g * 16;
-        float v[16];
-        if (p.dbg & 2) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = (float)i;
-        } else {
-          tmem_ld16(t_addr + c0, v);
-        }
-        const float4* b4 = reinterpret_cast<const float4*>(s_bias + c0);
-#pragma unroll
-        for (int i4 = 0; i4 < 4; ++i4) {
-          const float4 bb = b4[i4];
-          const float bv[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float x = v[i4 * 4 + k] + bv[k];
-            const float y = FAST == 1 ? fmaxf(x, x * alpha)
-                            : (FAST == 2 ? alpha * exp2f(-0.72134752f * fmaxf(x, 0.f))
-                                         : act_f(x, p.act, alpha));
-            v[i4 * 4 + k] = valid ? y : 0.f;
-          }
-        }
-        if (valid && !(p.dbg & 1)) {
-          if (!p.out_nchw) {
-            float4* o = reinterpret_cast<float4*>(p.out + pix * p.ld_out + c0);
-            o[0] = make_float4(v[0], v[1], v[2], v[3]);
-            o[1] = make_float4(v[4], v[5], v[6], v[7]);
-            o[2] = make_float4(v[8], v[9], v[10], v[11]);
-            o[3] = make_float4(v[12], v[13], v[14], v[15]);
-          } else {
-            const size_t hw = (size_t)p.nchw_stride;
-            float* o = p.out + ((size_t)n * p.Cout + c0) * hw + (size_t)gh * p.W + gw;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i * hw] = v[i];
-          }
-        }
-        if (NG > 0) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            rs[gi * 16 + i] += v[i];
-            rq[gi * 16 + i] = fmaf(v[i], v[i], rq[gi * 16 + i]);
-          }
-        } else if (do_stats) {
-          float w[32];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            w[i] = v[i];
-            w[16 + i] = v[i] * v[i];
-          }
-          const float tot = warp_transpose_sum32(w, lane);
-          my_stats[(lane < 16 ? 0 : p.Cout) + c0 + (lane & 15)] += tot;
-        }
-      };
-      if (NG > 0) {
-#pragma unroll
-        for (int g = 0; g < (NG > 0 ? NG : 1); ++g) group(g, g);
-      } else {
-        const int n_groups = p.Cout >> 4;
-#pragma unroll 1
-        for (int g = 0; g < n_groups; ++g) group(g, 0);
-      }
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&ctl->tmem_empty[acc]));
-    tl += kEpiGroups;
-  }
-  if (do_stats) {
-    if (NG > 0) {
-#pragma unroll
-      for (int g = 0; g < NG; ++g) {
-        float w[32];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          w[i] = rs[g * 16 + i];
-          w[16 + i] = rq[g * 16 + i];
-        }
-        const float tot = warp_transpose_sum32(w, lane);
-        my_stats[(lane < 16 ? 0 : p.Cout) + g * 16 + (lane & 15)] += tot;
-      }
-    }
-    __syncwarp();
-    for (int i = lane; i < 2 * p.Cout; i += 32) atomicAdd(p.stats + i, (double)my_stats[i]);
-  }
-}
-
 constexpr int kCtlBytes = 1024;     // SharedCtl, then the statistics / bias block
 static_assert(sizeof(SharedCtl) <= kCtlBytes, "SharedCtl must fit below the statistics block");
 
@@ -607,8 +565,8 @@ __global__ void __launch_bounds__(kThreads, 1)
   extern __shared__ __align__(1024) uint8_t smem[];
   SharedCtl* ctl = reinterpret_cast<SharedCtl*>(smem);
   float* s_stats = reinterpret_cast<float*>(smem + kCtlBytes);  // [4 warps][2][Cout]
-  const uint32_t stats_bytes = (kEpiGroups * kNumEpiWarps * 2 + 1) * p.Cout * sizeof(float);   // + bias copy
-  float* s_bias = s_stats + kEpiGroups * kNumEpiWarps * 2 * p.Cout;
+  const uint32_t stats_bytes = (kNumEpiWarps * 2 + 1) * p.Cout * sizeof(float);   // + bias copy
+  float* s_bias = s_stats + kNumEpiWarps * 2 * p.Cout;
   const uint32_t a_base = smem_u32(smem) + ((kCtlBytes + stats_bytes + 127) & ~127u);
   const uint32_t b_base = a_base + p.n_a * p.a_stage_bytes;
   const uint32_t raw_base = (b_base + p.w_bytes + 127) & ~127u;      // TMA mode (resident weights)
@@ -620,15 +578,11 @@ __global__ void __launch_bounds__(kThreads, 1)
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.n_a; ++i) {
       mbar_init(smem_u32(&ctl->full_a[i]), kNumLoadWarps / 2);
-      mbar_init(smem_u32(&ctl->empty_a[i]), 1);
+      mbar_init(smem_u32(&ctl->empty_a[i]), kNumEpiWarps);
     }
     for (int i = 0; i < p.n_b; ++i) {
       mbar_init(smem_u32(&ctl->full_b[i]), 1);
-      mbar_init(smem_u32(&ctl->empty_b[i]), 1);
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(smem_u32(&ctl->tmem_full[i]), 1);
-      mbar_init(smem_u32(&ctl->tmem_empty[i]), kNumEpiWarps);
+      mbar_init(smem_u32(&ctl->empty_b[i]), kNumEpiWarps);
     }
     for (int i = 0; i < kMaxRStages; ++i) {
       mbar_init(smem_u32(&ctl->raw_full[i]), 1);
@@ -637,26 +591,21 @@ __global__ void __launch_bounds__(kThreads, 1)
     mbar_init(smem_u32(&ctl->w_full), 1);
     fence_barrier_init();
   }
-  if (warp == kWgtWarp) tmem_alloc(smem_u32(&ctl->tmem_base), p.tmem_cols);
-  if (warp < kNumEpiWarps || warp >= kEpiBWarp) {
-    const int ew = warp < kNumEpiWarps ? warp : kNumEpiWarps + (warp - kEpiBWarp);
-    for (int i = lane; i < 2 * p.Cout; i += 32) s_stats[ew * 2 * p.Cout + i] = 0.f;
+  if (warp < kNumEpiWarps) {
+    for (int i = lane; i < 2 * p.Cout; i += 32) s_stats[warp * 2 * p.Cout + i] = 0.f;
     if (warp == 0)
       for (int i = lane; i < p.Cout; i += 32) s_bias[i] = p.bias ? __ldg(p.bias + i) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
 
   if (warp >= kFirstLoadWarp && warp < kEpiBWarp) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsLoad));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsLoad));
     // ===================== activation loaders =====================
-    // Two groups of 4 warps; group g stages the k-chunks with (global chunk counter & 1) == g, so
-    // two chunks are always in flight per SM.  Per thread the (halo row, halo col) of each of its
-    // <= kMaxU 16-byte elements is fixed for the whole kernel (no divisions in the loop); loads
-    // are issued branch-free from clamped addresses and masked afterwards, so the compiler keeps
-    // all of them in flight before the first use.
+    // Two groups of 4 warps; group g stages every k-chunk of the tiles with local index = g
+    // (mod 2), so two chunks are always in flight per SM.  Per thread the (halo row, halo col) of
+    // each of its <= kMaxU 16-byte elements is fixed for the whole kernel (no divisions in the
+    // loop); loads are issued branch-free from clamped addresses and masked afterwards, so the
+    // compiler keeps all of them in flight before the first use.
     const int grp = (warp - kFirstLoadWarp) >> 2;
     const int U = (p.HP * (p.KC >> 2) + kGroupThreads - 1) / kGroupThreads;   // <= kMaxU (plan)
     switch (U) {
@@ -698,7 +647,7 @@ __global__ void __launch_bounds__(kThreads, 1)
             const int h_org = th_i * kTileH - p.dil * (p.taps_h >> 1);
             const int w_org = tw_i * kTileW * p.sub - p.dil * (p.taps_w >> 1);
             for (int ch = 0; ch < p.n_chunks; ++ch) {
-              mbar_wait(bar_empty + (rr0 + rs) * 8, rph);
+              mbar_wait_quiet(bar_empty + (rr0 + rs) * 8, rph);
               const uint32_t bar = bar_full + (rr0 + rs) * 8;
               mbar_arrive_expect_tx(bar, p.raw_bytes);
               const int c = ch * p.KC;
@@ -721,7 +670,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           const int wmult = p.x3 ? 2 : 1;
           for (int ch = 0; ch < p.n_chunks; ++ch) {
             for (int t = 0; t < taps; ++t) {
-              mbar_wait(bar_empty_b + (ring0 + st) * 8, ph);
+              mbar_wait_quiet(bar_empty_b + (ring0 + st) * 8, ph);
               const uint32_t bar = bar_full_b + (ring0 + st) * 8;
               mbar_arrive_expect_tx(bar, b_stage);
               // piece (k-step s, kind, tap) of the blob lives at ((s*wmult + kind)*taps + tap);
@@ -738,56 +687,31 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
     __syncwarp();
-   } else if (warp == kMmaWarp || warp == kMmaWarp2) {
-    const int issuer = warp == kMmaWarp ? 0 : 1;
-    // ===================== MMA issuer =====================
-    // One elected thread issues every tcgen05.mma, so its instruction count per MMA bounds the
-    // kernel for the thin layers (an M128 x N16 x K8 MMA is 8 tensor-pipe cycles).  The loop nest
-    // (ty, tx, k-step) advances both descriptors by constant increments only.
-    if (elect_one()) {
-      const int ksteps = p.KC >> 3;
-      const bool res = p.w_resident != 0;
-#define AB_MMA_CASE(K, S, R) mma_issue_loop<K, S, R>(p, ctl, tmem_base, a_base, b_base, issuer)
-      if (p.sub == 1) {
-        if (res) { if (ksteps == 4) AB_MMA_CASE(4, 1, true); else if (ksteps == 2) AB_MMA_CASE(2, 1, true); else AB_MMA_CASE(1, 1, true); }
-        else     { if (ksteps == 4) AB_MMA_CASE(4, 1, false); else if (ksteps == 2) AB_MMA_CASE(2, 1, false); else AB_MMA_CASE(1, 1, false); }
-      } else {
-        if (res) { if (ksteps == 4) AB_MMA_CASE(4, 2, true); else if (ksteps == 2) AB_MMA_CASE(2, 2, true); else AB_MMA_CASE(1, 2, true); }
-        else     { if (ksteps == 4) AB_MMA_CASE(4, 2, false); else if (ksteps == 2) AB_MMA_CASE(2, 2, false); else AB_MMA_CASE(1, 2, false); }
-      }
-#undef AB_MMA_CASE
-    }
-    __syncwarp();
    }
   } else {
-    if (kEpiGroups == 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsEpi));
-    else asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsEpi));
-    // ===================== epilogue (kEpiGroups groups, group e <-> tiles e mod kEpiGroups) =====
-    const int eg = warp < kNumEpiWarps ? 0 : 1;
-    const bool fast = p.act == AB_ACT_LRELU && p.alpha >= 0.f && p.alpha <= 1.f;
-    const int ng = p.stats ? p.Cout >> 4 : 0;
-    if (fast) {
-      if (ng == 1) epilogue_loop<1, 1>(p, ctl, tmem_base, s_stats, s_bias, eg);
-      else if (ng == 2) epilogue_loop<2, 1>(p, ctl, tmem_base, s_stats, s_bias, eg);
-      else epilogue_loop<0, 1>(p, ctl, tmem_base, s_stats, s_bias, eg);
-    } else if (p.act == AB_ACT_RBF) {
-      epilogue_loop<0, 2>(p, ctl, tmem_base, s_stats, s_bias, eg);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsEpi));
+    // ===================== consumer: wgmma + epilogue =====================
+#define AB_CONS_CASE(NN, S) case NN: consumer_loop<NN, S>(p, ctl, a_base, b_base, s_stats, s_bias); break;
+    if (p.sub == 2) {
+      switch (p.nn) {
+        AB_CONS_CASE(16, 2) AB_CONS_CASE(32, 2) AB_CONS_CASE(48, 2) AB_CONS_CASE(64, 2)
+        default: __trap();
+      }
     } else {
-      epilogue_loop<0, 0>(p, ctl, tmem_base, s_stats, s_bias, eg);
+      switch (p.nn) {
+        AB_CONS_CASE(16, 1) AB_CONS_CASE(32, 1) AB_CONS_CASE(48, 1) AB_CONS_CASE(64, 1)
+        AB_CONS_CASE(80, 1) AB_CONS_CASE(96, 1) AB_CONS_CASE(112, 1) AB_CONS_CASE(128, 1)
+        default: __trap();
+      }
     }
+#undef AB_CONS_CASE
   }
-
-  tc_fence_before();
   __syncthreads();
-  if (warp == kWgtWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
 }
 
 // ---------------------------------------------------------------- weight packing (TF32 blobs)
 // blob[k-step s (8 channels)][tap][plane j (2)][n][4]  <-  W, RN-rounded to TF32.  One (s, tap)
-// piece is a ready-made UMMA K-major B operand for one tcgen05.mma (N rows x 8 k).
+// piece is a ready-made K-major B operand for one wgmma (N rows x 8 k).
 //   FWD  : B[n = co][k = ci]            = W[co][ci][ty][tx]
 //   DGRAD: B[n = ci][k = co] (roles swap) = W[co][ci][Th-1-ty][Tw-1-tx]
 // x3 (AB_MATH_TF32X3): blob[k-step][kind (main, corr)][tap][plane][n][4 words]: the main piece as
@@ -882,15 +806,12 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
     const int kb = atoi(e);
     if (kb >= 64 && kb <= 224) budget = kb * 1024;
   }
-  // Operand-ring preference (measured, tools/plan_ab.py, profiles/r02_plan_ab.md).  Every
-  // pipeline owns n_a/2 operand stages; with n_a = 2 the loader group and the issuing thread of
-  // a pipeline strictly alternate (stage -> MMA -> stage ...) and only the *other* pipeline hides
-  // the hand-over.  tf32x3 doubled the stage size and had silently dropped most 3x3 layers from
-  // n_a = 4 to 2: c6.0 977 -> 753 us, c2.1/c5.1 285 -> 226 us, c4.0 316 -> 272 us with the
-  // deeper ring.  It does NOT pay to buy the deeper ring with 8-channel k-chunks when the
-  // loaders are the heavy side (pooled sources, register-staged resident layers: c3.0 154 -> 170,
-  // c5.0 512 -> 528 us), so pass 0 of the search only drops to KC = 8 for streamed-weight layers
-  // with plain sources (bn.1 150 -> 136 us).
+  // Operand-ring preference.  Every pipeline owns n_a/2 operand stages; with n_a = 2 the loader
+  // group and the consumer strictly alternate on a pipeline (stage -> MMA -> stage ...) and only
+  // the *other* pipeline hides the hand-over.  Buying the deeper ring with 8-channel k-chunks does
+  // not pay when the loaders are the heavy side (pooled sources, register-staged resident
+  // layers), so pass 0 of the search only drops to KC = 8 for streamed-weight layers with plain
+  // sources.
   // bit 0: resident-weight plans prefer n_a = 4 over more raw TMA stages;
   // bit 1: streamed-weight plans prefer n_a = 4 over a larger k-chunk / more weight stages.
   int na4 = 3;
@@ -901,24 +822,20 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
   if (const char* e = getenv("ATOMAI_B200_MIN_NR")) min_nr = atoi(e) < 2 ? 2 : atoi(e);
   bool any_pool = false;
   for (int i = 0; i < S.nsrc; ++i) any_pool = any_pool || S.s[i].pool != 0;
-  const int stats_bytes = (((kEpiGroups * kNumEpiWarps * 2 + 1) * d->Cout * 4 + 127) & ~127) + kCtlBytes + 128;
+  const int stats_bytes = (((kNumEpiWarps * 2 + 1) * d->Cout * 4 + 127) & ~127) + kCtlBytes + 128;
   // Try, in order of preference: (resident weights, 1 sub-tile), (streamed weights, 2 sub-tiles
   // so that every weight stage feeds M = 256), (streamed, 1 sub-tile).
   // tuning hooks (bring-up only): ATOMAI_B200_PLAN="<attempt>,<KC>" pins the plan search
   int force_attempt = -1, force_kc = 0;
   if (const char* e = getenv("ATOMAI_B200_PLAN")) sscanf(e, "%d,%d", &force_attempt, &force_kc);
-  p->dbg = 0;
-  if (const char* e = getenv("ATOMAI_B200_DBG")) p->dbg = atoi(e);
   const char* e_tma = getenv("ATOMAI_B200_TMA");      // "0" pins the register-staged loaders
   const bool use_tma = !(e_tma && e_tma[0] == '0');
   bool ok = false;
-  // Resident weights that leave only n_a = 2 vs streamed weights with n_a = 4 (measured,
-  // profiles/r02_plan_ab.md): streaming wins only where the weight ring gets deep enough to cover
-  // the L2 latency — the two-source decoder convolution onto <= 32 channels (c5.0: 64 -> 32,
-  // 14 weight stages: 513 -> 425 us); with 6 stages it loses (c5.0 dgrad 339 -> 374, c3.0
-  // 155 -> 183 us).  So: for that layer class a resident plan must reach n_a = 4, else a streamed
-  // plan with >= 12 weight stages is preferred; the resident n_a = 2 plan stays the fallback.
-  // ATOMAI_B200_RES_NA4 = 0 disables, = 1 applies the rule to every layer (sweeps).
+  // Resident weights that leave only n_a = 2 vs streamed weights with n_a = 4: streaming wins only
+  // where the weight ring gets deep enough to cover the L2 latency, i.e. for the two-source
+  // decoder convolution onto <= 32 channels.  So: for that layer class a resident plan must reach
+  // n_a = 4, else a streamed plan with >= 12 weight stages is preferred; the resident n_a = 2 plan
+  // stays the fallback.  ATOMAI_B200_RES_NA4 = 0 disables, = 1 applies the rule to every layer.
   const char* e_strict = getenv("ATOMAI_B200_RES_NA4");
   int strict0 = (p->x3 && S.nsrc == 2 && !any_pool && taps == 9 && d->Cout <= 32) ? 1 : 0;
   if (e_strict) strict0 = e_strict[0] == '1' ? 1 : 0;
@@ -927,7 +844,7 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
     if (force_attempt >= 0 && attempt != force_attempt) continue;
     const int resident = attempt == 0;
     const int sub = attempt == 1 ? 2 : 1;
-    if (sub == 2 && (4 * d->Cout > 512 || d->W <= kTileW)) continue;
+    if (sub == 2 && (d->Cout > kMaxN / 2 || d->W <= kTileW)) continue;   // SUB * N accumulators
     p->tiles_h = (d->H + kTileH - 1) / kTileH;
     p->tiles_w = (d->W + kTileW * sub - 1) / (kTileW * sub);
     p->THp = kTileH + d->dil * (d->ks_h - 1);
@@ -953,7 +870,7 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
       if (resident) {
         avail -= (p->w_bytes + 127) & ~127;
       } else {
-        // weight stages: cover ~1.5 us of L2 latency, leave room for the activation stages
+        // weight stages: cover the L2 latency, leave room for the activation stages
         n_b = ((avail - need_a * a_stage) / b_stage) & ~1;      // two rings of n_b/2 stages
         if (n_b > kMaxBStages) n_b = kMaxBStages;
         if (n_b < (strict ? 12 : 4)) continue;
@@ -1008,10 +925,6 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
   p->num_tiles = d->N * p->tiles_h * p->tiles_w;
   p->n_chunks = S.Ctot / p->KC;
   AB_CHECK(p->plane_bytes / 16 < (1 << 14) && p->TWp < (1 << 14), "conv_tc: descriptor overflow");
-  p->n_acc = 4 * p->sub * d->Cout <= 512 ? 4 : 2;
-  int cols = 32;
-  while (cols < p->n_acc * p->sub * d->Cout) cols <<= 1;
-  p->tmem_cols = cols;
   *smem_bytes = stats_bytes + p->n_a * p->a_stage_bytes +
                 (p->w_resident ? ((p->w_bytes + 127) & ~127) : p->n_b * p->b_stage_bytes) +
                 p->n_r * p->raw_bytes + (p->tma ? 128 : 0);
@@ -1077,6 +990,7 @@ int ab_conv_tc_fwd(const ab_conv_t* d, const float* wblob, const float* bias, fl
   const int sms = ab_num_sms();
   const int grid = p.num_tiles < sms ? p.num_tiles : sms;
   if (grid == 0) return 0;
+  if (stats && ab_ordered_ws(stream, (int64_t)grid * 2 * kMaxN, 1, &p.red)) return 1;
   CUtensorMap tm0, tm1;
   memset(&tm0, 0, sizeof(tm0));
   memset(&tm1, 0, sizeof(tm1));
@@ -1084,7 +998,12 @@ int ab_conv_tc_fwd(const ab_conv_t* d, const float* wblob, const float* bias, fl
     if (make_src_tmap(p.S.s[0], p.N, p.H, p.W, p.KC, p.TWp, p.THp, &tm0)) return 1;
     if (p.S.nsrc > 1 && make_src_tmap(p.S.s[1], p.N, p.H, p.W, p.KC, p.TWp, p.THp, &tm1)) return 1;
   }
-  conv_tc_kernel<<<grid, kThreads, smem_bytes, stream>>>(p, tm0, tm1);
-  AB_LAUNCH_CHECK();
+  // one launch per <= 128 output channels (the consumer's accumulator registers)
+  for (int n0 = 0; n0 < d->Cout; n0 += kMaxN) {
+    p.n0 = n0;
+    p.nn = d->Cout - n0 < kMaxN ? d->Cout - n0 : kMaxN;
+    conv_tc_kernel<<<grid, kThreads, smem_bytes, stream>>>(p, tm0, tm1);
+    AB_LAUNCH_CHECK();
+  }
   return 0;
 }

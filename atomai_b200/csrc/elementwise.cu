@@ -2,8 +2,8 @@
 // LeakyReLU backward, 2x2 max-pool, bilinear/nearest x2 upsampling, gradient routing, the
 // DilatedBlock sum, losses and the fused multi-tensor Adam step.  All are coalesced along the
 // channel axis of the NHWC activations (float4 when C % 4 == 0) and grid-sized as a multiple of
-// the SM count.  Per-channel reductions go warp/CTA-local first and finish with one double
-// atomicAdd per (CTA, channel).
+// the SM count.  Per-channel reductions go warp/CTA-local first and finish with an ordered
+// cross-CTA sum in double per channel.
 //
 // Reference call sites: nn.BatchNorm2d atomai/nets/blocks.py:73; nn.LeakyReLU :70;
 // F.max_pool2d atomai/nets/fcnn.py:123-127; F.interpolate atomai/nets/blocks.py:130-131;
@@ -16,6 +16,11 @@
 namespace {
 
 constexpr int kT = 256;
+
+// workspace of an ordered cross-CTA sum of n values per CTA for a launch of grid_for() CTAs
+int red_ws(cudaStream_t stream, int n, Ordered* red) {
+  return ab_ordered_ws(stream, (int64_t)ab_num_sms() * 8 * n, 1, red);
+}
 
 inline int grid_for(int64_t work_items, int per_block = kT) {
   int64_t b = (work_items + per_block - 1) / per_block;
@@ -90,8 +95,11 @@ inline ChanLayout chan_layout(int C) {
   return l;
 }
 
+// The CTA's per-channel totals go into its slot of an ordered cross-CTA sum (common.cuh), so the
+// result does not depend on which CTA finishes first.
 __device__ __forceinline__ void block_chan_reduce2(float v1, float v2, int cx, int py, int CW,
-                                                   int R, int C, double* out1, double* out2) {
+                                                   int R, int C, double* out1, double* out2,
+                                                   const Ordered& red) {
   __shared__ float s1[kT], s2[kT];
   s1[py * CW + cx] = v1;
   s2[py * CW + cx] = v2;
@@ -102,16 +110,24 @@ __device__ __forceinline__ void block_chan_reduce2(float v1, float v2, int cx, i
       a += s1[r * CW + cx];
       b += s2[r * CW + cx];
     }
-    if (out1) atomicAdd(out1 + cx, (double)a);
-    if (out2) atomicAdd(out2 + cx, (double)b);
+    double* slot = ordered_slot(red, 0, gridDim.x, blockIdx.x, 2 * C);
+    slot[cx] = a;
+    slot[C + cx] = b;
   }
+  __shared__ unsigned s_last;
+  ordered_finish(red, 0, gridDim.x, 2 * C, threadIdx.x, kT, gridDim.x, [] { __syncthreads(); },
+                 [&](int i, double v) {
+                   double* o = i < C ? out1 : out2;
+                   if (o) o[i < C ? i : i - C] += v;
+                 },
+                 &s_last);
 }
 
 __global__ void __launch_bounds__(kT) bn_bwd_reduce_kernel(const float* __restrict__ dy, int ld_dy,
                                                            const float* __restrict__ a, int ld_a,
                                                            const float* mean, const float* invstd,
                                                            int64_t npix, int C, int CW, int R,
-                                                           double* sums) {
+                                                           double* sums, Ordered red) {
   const int cx = threadIdx.x % CW, py = threadIdx.x / CW;
   float s1 = 0.f, s2 = 0.f;
   if (cx < C) {
@@ -123,7 +139,7 @@ __global__ void __launch_bounds__(kT) bn_bwd_reduce_kernel(const float* __restri
       s2 = fmaf(g, xh, s2);
     }
   }
-  block_chan_reduce2(s1, s2, cx, py, CW, R, C, sums, sums + C);
+  block_chan_reduce2(s1, s2, cx, py, CW, R, C, sums, sums + C, red);
 }
 
 __global__ void __launch_bounds__(kT)
@@ -131,7 +147,7 @@ __global__ void __launch_bounds__(kT)
                         int ld_a, const float* mean, const float* invstd, const float* scale,
                         const double* sums, double count, const float* __restrict__ extra,
                         int ld_extra, int act, float alpha, float* __restrict__ dpre, int ld_dpre,
-                        double* dbias, int64_t npix, int C, int CW, int R) {
+                        double* dbias, int64_t npix, int C, int CW, int R, Ordered red) {
   const int cx = threadIdx.x % CW, py = threadIdx.x / CW;
   float sb = 0.f;
   if (cx < C) {
@@ -161,7 +177,7 @@ __global__ void __launch_bounds__(kT)
       sb += d;
     }
   }
-  if (dbias) block_chan_reduce2(sb, 0.f, cx, py, CW, R, C, dbias, nullptr);
+  if (dbias) block_chan_reduce2(sb, 0.f, cx, py, CW, R, C, dbias, nullptr, red);
 }
 
 // ---------------------------------------------------------------- 2x2 max pool
@@ -340,7 +356,7 @@ __global__ void __launch_bounds__(kT) ce_kernel(const float* __restrict__ logits
                                                 const int64_t* __restrict__ labels, int64_t npix,
                                                 int C, double* loss_sum,
                                                 float* __restrict__ dlogits, int ld_d,
-                                                float gscale, const float* gscale_dev) {
+                                                float gscale, const float* gscale_dev, Ordered red) {
   float local = 0.f;
   if (gscale_dev) gscale *= __ldg(gscale_dev);
   for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < npix;
@@ -361,15 +377,19 @@ __global__ void __launch_bounds__(kT) ce_kernel(const float* __restrict__ logits
       }
     }
   }
-  __shared__ float red[kT / 32];
+  __shared__ float wred[kT / 32];
   const float ws = warp_sum(local);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ws;
+  if ((threadIdx.x & 31) == 0) wred[threadIdx.x >> 5] = ws;
   __syncthreads();
   if (threadIdx.x == 0) {
     float t = 0.f;
-    for (int i = 0; i < kT / 32; ++i) t += red[i];
-    if (loss_sum) atomicAdd(loss_sum, (double)t);
+    for (int i = 0; i < kT / 32; ++i) t += wred[i];
+    if (loss_sum) ordered_slot(red, 0, gridDim.x, blockIdx.x, 1)[0] = (double)t;
   }
+  __shared__ unsigned s_last;
+  if (loss_sum)
+    ordered_finish(red, 0, gridDim.x, 1, threadIdx.x, kT, gridDim.x, [] { __syncthreads(); },
+                   [&](int, double v) { *loss_sum += v; }, &s_last);
 }
 
 __global__ void __launch_bounds__(kT) pointwise_loss_kernel(const float* __restrict__ pred,
@@ -377,7 +397,7 @@ __global__ void __launch_bounds__(kT) pointwise_loss_kernel(const float* __restr
                                                             int64_t n, int kind, double* loss_sum,
                                                             float* __restrict__ dpred,
                                                             float gscale,
-                                                            const float* gscale_dev) {
+                                                            const float* gscale_dev, Ordered red) {
   float local = 0.f;
   if (gscale_dev) gscale *= __ldg(gscale_dev);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n;
@@ -392,21 +412,25 @@ __global__ void __launch_bounds__(kT) pointwise_loss_kernel(const float* __restr
       if (dpred) dpred[i] = (1.f / (1.f + __expf(-x)) - t) * gscale;
     }
   }
-  __shared__ float red[kT / 32];
+  __shared__ float wred[kT / 32];
   const float ws = warp_sum(local);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ws;
+  if ((threadIdx.x & 31) == 0) wred[threadIdx.x >> 5] = ws;
   __syncthreads();
   if (threadIdx.x == 0) {
     float t = 0.f;
-    for (int i = 0; i < kT / 32; ++i) t += red[i];
-    if (loss_sum) atomicAdd(loss_sum, (double)t);
+    for (int i = 0; i < kT / 32; ++i) t += wred[i];
+    if (loss_sum) ordered_slot(red, 0, gridDim.x, blockIdx.x, 1)[0] = (double)t;
   }
+  __shared__ unsigned s_last;
+  if (loss_sum)
+    ordered_finish(red, 0, gridDim.x, 1, threadIdx.x, kT, gridDim.x, [] { __syncthreads(); },
+                   [&](int, double v) { *loss_sum += v; }, &s_last);
 }
 
 __global__ void __launch_bounds__(kT) sqerr_kernel(const float* __restrict__ x,
                                                    const float* __restrict__ xhat, int64_t n,
                                                    double* out, float* __restrict__ dxhat,
-                                                   float gscale, const float* gscale_dev) {
+                                                   float gscale, const float* gscale_dev, Ordered red) {
   float local = 0.f;
   if (gscale_dev) gscale *= __ldg(gscale_dev);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n;
@@ -415,15 +439,19 @@ __global__ void __launch_bounds__(kT) sqerr_kernel(const float* __restrict__ x,
     local = fmaf(d, d, local);
     if (dxhat) dxhat[i] = d * gscale;
   }
-  __shared__ float red[kT / 32];
+  __shared__ float wred[kT / 32];
   const float ws = warp_sum(local);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ws;
+  if ((threadIdx.x & 31) == 0) wred[threadIdx.x >> 5] = ws;
   __syncthreads();
   if (threadIdx.x == 0) {
     float t = 0.f;
-    for (int i = 0; i < kT / 32; ++i) t += red[i];
-    if (out) atomicAdd(out, 0.5 * (double)t);
+    for (int i = 0; i < kT / 32; ++i) t += wred[i];
+    if (out) ordered_slot(red, 0, gridDim.x, blockIdx.x, 1)[0] = 0.5 * (double)t;
   }
+  __shared__ unsigned s_last;
+  if (out)
+    ordered_finish(red, 0, gridDim.x, 1, threadIdx.x, kT, gridDim.x, [] { __syncthreads(); },
+                   [&](int, double v) { *out += v; }, &s_last);
 }
 
 // ---------------------------------------------------------------- Adam (multi-tensor)
@@ -506,7 +534,7 @@ __global__ void __launch_bounds__(kT) add_slice_vec_kernel(const float* __restri
 
 // per-channel reductions: thread = (c4 lane cx, pixel row py), CW4 = pow2 >= C4, R = 256 / CW4
 __device__ __forceinline__ void block_chan_reduce_vec(float4 v1, float4 v2, int cx, int py, int CW, int R, int C4,
-                                                      double* out1, double* out2) {
+                                                      double* out1, double* out2, const Ordered& red) {
   __shared__ float4 s1[kT], s2[kT];
   s1[py * CW + cx] = v1;
   s2[py * CW + cx] = v2;
@@ -514,16 +542,24 @@ __device__ __forceinline__ void block_chan_reduce_vec(float4 v1, float4 v2, int 
   if (py == 0 && cx < C4) {
     float4 a = make_float4(0, 0, 0, 0), b = a;
     for (int r = 0; r < R; ++r) { a = f4add(a, s1[r * CW + cx]); b = f4add(b, s2[r * CW + cx]); }
-    if (out1) { atomicAdd(out1 + cx * 4, (double)a.x); atomicAdd(out1 + cx * 4 + 1, (double)a.y);
-                atomicAdd(out1 + cx * 4 + 2, (double)a.z); atomicAdd(out1 + cx * 4 + 3, (double)a.w); }
-    if (out2) { atomicAdd(out2 + cx * 4, (double)b.x); atomicAdd(out2 + cx * 4 + 1, (double)b.y);
-                atomicAdd(out2 + cx * 4 + 2, (double)b.z); atomicAdd(out2 + cx * 4 + 3, (double)b.w); }
+    double* slot = ordered_slot(red, 0, gridDim.x, blockIdx.x, 8 * C4);
+    slot[cx * 4] = a.x; slot[cx * 4 + 1] = a.y; slot[cx * 4 + 2] = a.z; slot[cx * 4 + 3] = a.w;
+    double* s2_ = slot + 4 * C4;
+    s2_[cx * 4] = b.x; s2_[cx * 4 + 1] = b.y; s2_[cx * 4 + 2] = b.z; s2_[cx * 4 + 3] = b.w;
   }
+  __shared__ unsigned s_last;
+  const int C = 4 * C4;
+  ordered_finish(red, 0, gridDim.x, 2 * C, threadIdx.x, kT, gridDim.x, [] { __syncthreads(); },
+                 [&](int i, double v) {
+                   double* o = i < C ? out1 : out2;
+                   if (o) o[i < C ? i : i - C] += v;
+                 },
+                 &s_last);
 }
 
 __global__ void __launch_bounds__(kT) bn_bwd_reduce_vec_kernel(const float* __restrict__ dy, int ld_dy, const float* __restrict__ a,
                                          int ld_a, const float* mean, const float* invstd, int64_t npix, int C4,
-                                         int CW, int R, double* sums) {
+                                         int CW, int R, double* sums, Ordered red) {
   const int cx = threadIdx.x % CW, py = threadIdx.x / CW;
   float4 s1 = make_float4(0, 0, 0, 0), s2 = s1;
   if (cx < C4) {
@@ -535,7 +571,7 @@ __global__ void __launch_bounds__(kT) bn_bwd_reduce_vec_kernel(const float* __re
       s2.z = fmaf(g.z, (av.z - m.z) * is.z, s2.z); s2.w = fmaf(g.w, (av.w - m.w) * is.w, s2.w);
     }
   }
-  block_chan_reduce_vec(s1, s2, cx, py, CW, R, C4, sums, sums + C4 * 4);
+  block_chan_reduce_vec(s1, s2, cx, py, CW, R, C4, sums, sums + C4 * 4, red);
 }
 
 __device__ __forceinline__ float bwd1(float g, float av, bool bn, float m, float is, float sc, float k1, float k2,
@@ -549,7 +585,7 @@ __global__ void __launch_bounds__(kT) bn_lrelu_bwd_vec_kernel(const float* __res
                                         const float* mean, const float* invstd, const float* scale, const double* sums,
                                         double count, const float* __restrict__ extra, int ld_extra, int act, float alpha,
                                         float* __restrict__ dpre, int ld_dpre, double* dbias, int64_t npix, int C4,
-                                        int CW, int R) {
+                                        int CW, int R, Ordered red) {
   const int cx = threadIdx.x % CW, py = threadIdx.x / CW;
   float4 sb = make_float4(0, 0, 0, 0);
   if (cx < C4) {
@@ -574,7 +610,7 @@ __global__ void __launch_bounds__(kT) bn_lrelu_bwd_vec_kernel(const float* __res
       sb = f4add(sb, d);
     }
   }
-  if (dbias) block_chan_reduce_vec(sb, make_float4(0, 0, 0, 0), cx, py, CW, R, C4, dbias, nullptr);
+  if (dbias) block_chan_reduce_vec(sb, make_float4(0, 0, 0, 0), cx, py, CW, R, C4, dbias, nullptr, red);
 }
 
 __global__ void __launch_bounds__(kT) pool_fwd_vec_kernel(const float* __restrict__ a, int ld_a, const float* scale, const float* shift,
@@ -608,7 +644,7 @@ template <bool STATS>
 __global__ void __launch_bounds__(kT) pool_bwd_vec_kernel(const float* __restrict__ dp, int ld_dp, const float* __restrict__ a, int ld_a,
                                     const float* scale, const float* shift, float* __restrict__ df, int ld_df,
                                     int accumulate, int Ho, int Wo, uint32_t total, VIdx ix,
-                                    const float* mean, const float* invstd, double* sums) {
+                                    const float* mean, const float* invstd, double* sums, Ordered red) {
   const int W2 = 2 * Wo;
   float4 s1 = make_float4(0, 0, 0, 0), s2 = s1, mu = s1, is = s1;
   if (STATS) {
@@ -648,7 +684,7 @@ __global__ void __launch_bounds__(kT) pool_bwd_vec_kernel(const float* __restric
   }
   if (STATS) {
     const int C4 = ix.C4, cx = threadIdx.x & (C4 - 1), py = threadIdx.x / C4;
-    block_chan_reduce_vec(s1, s2, cx, py, C4, kT / C4, C4, sums, sums + C4 * 4);
+    block_chan_reduce_vec(s1, s2, cx, py, C4, kT / C4, C4, sums, sums + C4 * 4, red);
   }
 }
 
@@ -788,16 +824,20 @@ int atomai_b200_bn_bwd_reduce(const float* dy, int ld_dy, const float* a, int ld
   if (npix == 0) return 0;
   if (C <= 4 * kT && vec_ok(C, {dy, a, mean, invstd}, {ld_dy, ld_a}, npix)) {
     const ChanLayout l4 = chan_layout(C / 4);
+    Ordered red;
+    if (red_ws(STREAM, 2 * C, &red)) return 1;
     bn_bwd_reduce_vec_kernel<<<grid_for(npix, l4.R * 8), kT, 0, STREAM>>>(
-        dy, ld_dy, a, ld_a, mean, invstd, npix, C / 4, l4.CW, l4.R, sums);
+        dy, ld_dy, a, ld_a, mean, invstd, npix, C / 4, l4.CW, l4.R, sums, red);
     AB_LAUNCH_CHECK();
     return 0;
   }
   AB_CHECK(C <= kT, "bn_bwd_reduce: C=%d unsupported (max %d, or %d when C %% 4 == 0)", C, kT, 4 * kT);
   const ChanLayout l = chan_layout(C);
+  Ordered red;
+  if (red_ws(STREAM, 2 * C, &red)) return 1;
   bn_bwd_reduce_kernel<<<grid_for(npix, l.R * 8), kT, 0, STREAM>>>(dy, ld_dy, a, ld_a, mean,
                                                                   invstd, npix, C, l.CW, l.R,
-                                                                  sums);
+                                                                  sums, red);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -808,11 +848,13 @@ int atomai_b200_bn_lrelu_bwd(const float* dy, int ld_dy, const float* a, int ld_
                              int act, float lrelu, float* dpre, int ld_dpre, double* dbias,
                              int64_t npix, int C, void* stream) {
   if (npix == 0) return 0;
+  Ordered red = {nullptr, nullptr};
+  if (dbias && red_ws(STREAM, 2 * C, &red)) return 1;
   if (C <= 4 * kT && vec_ok(C, {dy, a, mean, invstd, scale, extra, dpre}, {dy ? ld_dy : 0, ld_a, extra ? ld_extra : 0, ld_dpre}, npix)) {
     const ChanLayout l4 = chan_layout(C / 4);
     bn_lrelu_bwd_vec_kernel<<<grid_for(npix, l4.R * 8), kT, 0, STREAM>>>(
         dy, ld_dy, a, ld_a, mean, invstd, scale, sums, count, extra, ld_extra, act, lrelu, dpre,
-        ld_dpre, dbias, npix, C / 4, l4.CW, l4.R);
+        ld_dpre, dbias, npix, C / 4, l4.CW, l4.R, red);
     AB_LAUNCH_CHECK();
     return 0;
   }
@@ -820,7 +862,7 @@ int atomai_b200_bn_lrelu_bwd(const float* dy, int ld_dy, const float* a, int ld_
   const ChanLayout l = chan_layout(C);
   bn_lrelu_bwd_kernel<<<grid_for(npix, l.R * 8), kT, 0, STREAM>>>(
       dy, ld_dy, a, ld_a, mean, invstd, scale, sums, count, extra, ld_extra, act, lrelu, dpre,
-      ld_dpre, dbias, npix, C, l.CW, l.R);
+      ld_dpre, dbias, npix, C, l.CW, l.R, red);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -854,13 +896,15 @@ int atomai_b200_pool2x2_bwd_bn(const float* dp, int ld_dp, const float* a, int l
     if (stats) {
       AB_CHECK(ix.shift >= 0 && ix.C4 <= kT && ((uintptr_t)mean & 15) == 0 && ((uintptr_t)invstd & 15) == 0,
                "pool2x2_bwd_bn: fused statistics need C/4 = power of two <= %d (C=%d)", kT, C);
+      Ordered red;
+      if (red_ws(STREAM, 2 * C, &red)) return 1;
       pool_bwd_vec_kernel<true><<<grid_for(total / 4), kT, 0, STREAM>>>(
           dp, ld_dp, a, ld_a, scale, shift, dfull, ld_df, accumulate, Ho, Wo, (uint32_t)(total / 4), ix,
-          mean, invstd, sums);
+          mean, invstd, sums, red);
     } else {
       pool_bwd_vec_kernel<false><<<grid_for(total / 4), kT, 0, STREAM>>>(
           dp, ld_dp, a, ld_a, scale, shift, dfull, ld_df, accumulate, Ho, Wo, (uint32_t)(total / 4), ix,
-          nullptr, nullptr, nullptr);
+          nullptr, nullptr, nullptr, Ordered{nullptr, nullptr});
     }
     AB_LAUNCH_CHECK();
     return 0;
@@ -948,8 +992,10 @@ int atomai_b200_ce_fwd_bwd(const float* logits, int ld, const int64_t* labels, i
                            double* loss_sum, float* dlogits, int ld_d, float gscale,
                            const float* gscale_dev, void* stream) {
   if (npix == 0) return 0;
+  Ordered red = {nullptr, nullptr};
+  if (loss_sum && red_ws(STREAM, 1, &red)) return 1;
   ce_kernel<<<grid_for(npix), kT, 0, STREAM>>>(logits, ld, labels, npix, C, loss_sum, dlogits,
-                                               ld_d, gscale, gscale_dev);
+                                               ld_d, gscale, gscale_dev, red);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -959,8 +1005,10 @@ int atomai_b200_pointwise_loss(const float* pred, const float* target, int64_t n
                                const float* gscale_dev, void* stream) {
   AB_CHECK(kind == 0 || kind == 1, "pointwise_loss: kind=%d", kind);
   if (n == 0) return 0;
+  Ordered red = {nullptr, nullptr};
+  if (loss_sum && red_ws(STREAM, 1, &red)) return 1;
   pointwise_loss_kernel<<<grid_for(n), kT, 0, STREAM>>>(pred, target, n, kind, loss_sum, dpred,
-                                                        gscale, gscale_dev);
+                                                        gscale, gscale_dev, red);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -968,7 +1016,9 @@ int atomai_b200_pointwise_loss(const float* pred, const float* target, int64_t n
 int atomai_b200_sqerr_reduce(const float* x, const float* xhat, int64_t n, double* out,
                              float* dxhat, float gscale, const float* gscale_dev, void* stream) {
   if (n == 0) return 0;
-  sqerr_kernel<<<grid_for(n), kT, 0, STREAM>>>(x, xhat, n, out, dxhat, gscale, gscale_dev);
+  Ordered red = {nullptr, nullptr};
+  if (out && red_ws(STREAM, 1, &red)) return 1;
+  sqerr_kernel<<<grid_for(n), kT, 0, STREAM>>>(x, xhat, n, out, dxhat, gscale, gscale_dev, red);
   AB_LAUNCH_CHECK();
   return 0;
 }

@@ -2,9 +2,9 @@
 // The squared distance is ONE contraction over augmented operands,
 //     a' = [a/l, ||a/l||^2, 1, 0..]   b' = [-2 b/l, 1, ||b/l||^2, 0..]   =>  a'.b' = ||a/l - b/l||^2
 // (row norms by warp shuffles while scaling), so the -2ab^T term, both norms and the
-// exponentiation ride on the tcgen05 convolution kernel as a 1x1 convolution with an RBF /
-// Matern "activation" in its TMEM epilogue: x1 rows = pixels of a (1, n1/8, 8, K') image, column
-// blocks of <= 256 rows of x2 = output channels.  The n1 x n2 matrix is written exactly once.
+// exponentiation ride on the tensor-core convolution kernel as a 1x1 convolution with an RBF /
+// Matern "activation" in its register epilogue: x1 rows = pixels of a (1, n1/8, 8, K') image, column
+// blocks of <= 128 rows of x2 = output channels.  The n1 x n2 matrix is written exactly once.
 // AB_MATH_FP32 (and the < 8-row / < 16-column remainders of the tensor path) use the exact FFMA
 // tile kernel below.
 // RBF / Matern-2.5 / outputscale follow gpytorch's public kernel definitions as configured at
@@ -23,7 +23,7 @@ int ab_conv_tc_fwd(const ab_conv_t* d, const float* wblob, const float* bias, fl
 namespace {
 
 constexpr int TM = 64, TN = 64, TK = 16, GT = 256;
-constexpr int kColBlock = 256;      // max output channels (rows of K) per tcgen05 launch
+constexpr int kColBlock = 128;      // max output channels (rows of K) per tensor-core launch
 
 // one warp per row: out[row] = [x*inv_ls * fac, (side 0: |.|^2, 1) | (side 1: 1, |.|^2), 0-pad]
 __global__ void augment_kernel(const float* __restrict__ x, const float* __restrict__ inv_ls,
@@ -154,10 +154,10 @@ extern "C" int atomai_b200_gram(const float* x1, const float* x2, const float* i
     n2m = n2 & ~7;
   }
   if (n1m > 0 && n2m > 0) {
-    // tensor path: the rows of x2 are the pixels of a (1, n2m/8, 8, K') image, row blocks of <= 256
+    // tensor path: the rows of x2 are the pixels of a (1, n2m/8, 8, K') image, row blocks of <= 128
     // rows of x1 the output channels, stored "NCHW" with the channel pitch = ldk: lane l of an
     // epilogue warp holds K[r][c + l], so every store instruction writes 128 contiguous bytes of a
-    // row of K (the NHWC form wrote 16 B to 32 different rows per instruction: 1.1 TB/s, round 2)
+    // row of K (the NHWC form would write 16 B to 32 different rows per instruction)
     ab_conv_t cd;
     memset(&cd, 0, sizeof(cd));
     cd.N = 1; cd.H = n2m / 8; cd.W = 8;
@@ -165,8 +165,8 @@ extern "C" int atomai_b200_gram(const float* x1, const float* x2, const float* i
     cd.src[0].ptr = b; cd.src[0].C = Kp; cd.src[0].ld = Kp;
     cd.lrelu = outputscale; cd.math = math; cd.act = act; cd.out_nchw = 1;
     const int x3 = math == AB_MATH_TF32X3;
-    // rows of K per launch (measured, 50k x 50k x 128: 256 rows 1.18-1.24 TB/s, 128 rows 0.77-0.95,
-    // 64 rows 0.51-0.56 — wide N amortises the A-operand reads and the per-tile handshakes)
+    // rows of K per launch: as wide as the consumer's accumulator registers allow — wide N amortises
+    // the A-operand reads and the per-tile handshakes
     int blk = kColBlock;
     if (const char* e = getenv("ATOMAI_B200_GRAM_BLOCK")) blk = atoi(e);
     if (blk < 16 || blk > kColBlock || blk % 16 != 0) blk = kColBlock;

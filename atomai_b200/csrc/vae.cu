@@ -104,7 +104,7 @@ __global__ void bias_fill_kernel(float* C, int64_t c_sm, int M, int N, const flo
 // The latent heads of the VAE / ImSpec encoders (atomai/nets/ed.py:64,273-274: 262144..524288
 // inputs -> 2..13 outputs) are pure HBM streams over the activations: B x K floats read once,
 // a handful of outputs.  The 64x64 GEMM tile above wastes 59/64 of its B-operand lanes on them and
-// reads x in 64-byte pieces (measured 312-482 us per call, 27-31 % of an rVAE / ImSpec step);
+// reads x in 64-byte pieces;
 // these kernels read x / write dx as whole rows of float4 and keep the O-wide side in shared
 // memory or registers.
 constexpr int SK_T = 256;          // threads

@@ -1,42 +1,30 @@
-// wgrad_tc.cu — convolution weight gradient on tcgen05 (TF32 operands, fp32 accumulate in TMEM).
+// wgrad_tc.cu — convolution weight gradient on the Hopper tensor cores (wgmma, TF32 operands, fp32
+// accumulators in registers).
 //
 //   dW[co][ci][ty][tx] = sum_p dy[p][co] * x[p + (ty, tx) * dil][ci]        (SURVEY.md §2.4 K7)
 //
-// The reduction (GEMM K) runs over pixels, and both operands are contiguous along their channel
-// axis in NHWC memory, i.e. "MN-major" for the tensor core.  For 32-bit operands the only legal
-// MN-major shared-memory layout is SWIZZLE_128B_BASE32B: rows = k (pixels) at a 128 B pitch, 32
-// channels per row, the four 32 B chunks of a row XOR-ed with (row index mod 4) — which is
-// exactly a pixel-major NHWC tile.  The swizzle is a function of the absolute shared-memory
-// address (pinned by the selftest variants >= 8 / >= 32), so a tap is only a different start
-// address into the x halo tile, and one tcgen05.mma consumes 8 pixels (one row of a 16 x 8 tile).
-//
-// GEMM per kernel row ty:  D_ty[M = 128][N = co] += A[M][K = 8 px] * B[N][K]^T   with
-//   B = dy tile           [32-channel chunk][128 px][128 B]       (LBO = chunk stride)
-//   A = x halo tile, M = 4 chunks of 32 rows:
-//        taps_w > 1 ("tap-stacked"): chunk c = the SAME 32 input channels shifted by c*dil pixels,
-//                    i.e. LBO = dil * 128 B — the horizontal taps ride on the M axis, so a 3x3
-//                    kernel costs 3 x 16 MMAs per tile instead of 9 x 16, and N = Cout is not
-//                    padded to 128 (chunk 3 of a 3-wide kernel is a don't-care view);
-//        taps_w == 1: chunk c = input channels 32c..32c+31 (LBO = chunk stride), CTA owns 128 ci.
-// A CTA owns one input-channel block, one block of <= 128 output channels and a contiguous range
-// of pixel tiles; its taps_h x N accumulators stay in TMEM for the whole kernel and are flushed
-// once, with atomics, into dW (OIHW).  Warp roles: 4 MMA issue, 5 TMEM alloc, 8-11 / 12-15 / 0-3
-// three loader groups feeding a ring of shared-memory stages (setmaxnreg moves registers to
-// them); warps 0-3 also flush the accumulators at the end.
+// The reduction (GEMM K) runs over pixels.  wgmma reads 32-bit operands K-major only, so the
+// loaders transpose the channel-contiguous NHWC data while they stage it: a tile of 64 pixels
+// (8 x 8) becomes, per operand, rows = channels with the pixels along K, stored as no-swizzle core
+// matrices (8 rows x 4 pixels, LBO = 128 B between neighbouring pixel quads, SBO = one padded
+// 8-row group).  One CTA is one warpgroup and owns one tap, one block of 64 output channels (M),
+// one block of CIB input channels (N) and a contiguous range of pixel tiles; the x tile it stages
+// is already shifted by its tap, so every tap is the same GEMM D[co][ci] += dy^T x over the range.
+// The accumulators are flushed once into dW (OIHW), summed over the ranges in a fixed order.
+// Staging of tile i + 1 (global loads, TF32 rounding, x3 split) overlaps the MMAs of tile i through a two-stage ring.
 //
 // Replaces autograd's cuDNN bwd-filter behind loss.backward(), atomai/trainers/trainer.py:206.
 #include <cstdlib>
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int kTileH = 16, kTileW = 8;
-constexpr int kNumEpiWarps = 4, kMmaWarp = 4, kAllocWarp = 5, kFirstLoadWarp = 8;
-constexpr int kGroupThreads = 128;
-constexpr int kThreads = 512;                                     // 4 warpgroups
-constexpr int kRegsMma = 48, kRegsLoad = 152;                    // setmaxnreg re-balancing (3 x 152 + 48)
-constexpr int kMaxStages = 6;
-constexpr int kChunk = 128 * 128;             // bytes of one [128 px][32 ch] chunk of the dy tile
+constexpr int kTile = 8;                      // 8 x 8 pixel tiles: K = 64 per stage
+constexpr int kPix = kTile * kTile;
+constexpr int kThreads = 128;                 // one warpgroup
+constexpr int kM = 64;                        // output channels per CTA (wgmma M)
+constexpr int kSbo = (kPix / 4) * 128 + 32;   // one 8-row group: 16 pixel quads, padded (bank spread)
 
 struct WgradTcParams {
   SrcSet S;
@@ -46,1080 +34,146 @@ struct WgradTcParams {
   int ld_dy;
   float* dw;
   int tiles_h, tiles_w, num_tiles;
-  int cib;               // input channels per CTA: 32 (tap-stacked) or 128 (taps_w == 1)
-  int n_cc;              // input-channel blocks
-  int co_blocks;         // ceil(Cout / 128)
-  int ranges;            // pixel-tile ranges per (cc, co_block)
-  int TWp, THp, HP;
-  int x_chunk;           // taps_w == 1: bytes between 32-channel chunks of the x tile
-  int x_bytes, stage_bytes;
-  int n_stages;          // shared-memory ring depth (2..kMaxStages)
-  int fs;                // "fully stacked": Cout <= 32, the kernel rows ride on N (one MMA / halo row)
-  int dpad;              // fs: zero rows in front of / behind the dy tile = (taps_h - 1) * dil
-  int tmem_cols;
-  int x3;                // AB_MATH_TF32X3: a stage holds [x_hi][x_lo][dy_hi][dy_lo] (each value split into
-                         // rn_tf32(v) and the exact remainder) and every MMA is issued for the three
-                         // pairs (x_hi, dy_hi), (x_lo, dy_hi), (x_hi, dy_lo)
-  int dy_bytes;          // bytes of one dy tile inside a stage
-  int cob;               // output channels per CTA (128, or 64 when two stages would not fit)
-  int interleave;        // tile order (see the kernel)
-  int l2_prefetch;       // experiment (ATOMAI_B200_WGRAD_PF=1): loaders prefetch their next tile into L2;
-                         // measured SLOWER (4.37 vs 3.89 ms over the Unet's 15 layers): the loaders are
-                         // bound by instruction issue / the LSU pipe, not by DRAM latency — default off
-  int rt_loader;         // bring-up only (ATOMAI_B200_WGRAD_LOADER=1): run-time element loader everywhere
-  int legacy_loader;     // bring-up only (ATOMAI_B200_WGRAD_LOADER=0): the thread = pixel loaders
+  int cib;               // input channels per CTA (wgmma N: 16, 32 or 64)
+  int n_cib, n_cob;      // input / output channel blocks
+  int ranges;            // pixel-tile ranges per (tap, co block, ci block)
+  int a_bytes, b_bytes;  // one operand part (dy^T / x^T) of a stage
+  int stage_bytes;       // [dy_hi][x_hi] (x3: [dy_hi][dy_lo][x_hi][x_lo])
+  int x3;                // AB_MATH_TF32X3: every value split into rn_tf32(v) and the exact remainder;
+                         // per k-step the pairs (hi, hi), (lo, hi), (hi, lo) are issued
+  Ordered red;           // per (tap, channel block pair): ordered sum of the ranges' partial dW
 };
 
-struct __align__(8) Ctl {
-  uint64_t full[kMaxStages], empty[kMaxStages], done;
-  uint32_t tmem_base, pad;
-};
-
-__device__ __forceinline__ void sts128u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c,
-                                        uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c),
-               "r"(d)
-               : "memory");
-}
 // RN-to-TF32: the tensor core reads the upper 19 bits only (see conv_tc.cu tf32_bits)
 __device__ __forceinline__ uint32_t tf32b(float x) { return __float_as_uint(x) + 0x1000u; }
-// x3 operand part: the value itself (RN happens in tf32b) or its exact fp32 remainder x - rn_tf32(x)
-__device__ __forceinline__ float part(float x, bool lo) {
-  return lo ? x - __uint_as_float(tf32b(x) & 0xFFFFE000u) : x;
+__device__ __forceinline__ float lo_part(float x) {
+  return x - __uint_as_float(tf32b(x) & 0xFFFFE000u);
 }
-__device__ __forceinline__ float4 part4(float4 x, bool lo) {
-  return make_float4(part(x.x, lo), part(x.y, lo), part(x.z, lo), part(x.w, lo));
+// byte offset of (row r, pixel k) in the K-major core-matrix layout of one operand part
+__device__ __forceinline__ uint32_t kmaj_off(int r, int k) {
+  return (uint32_t)((r >> 3) * kSbo + (k >> 2) * 128 + (r & 7) * 16 + (k & 3) * 4);
 }
-// exact e / P for e < 65536 (mul = ceil(2^32 / P), P >= 2)
-__device__ __forceinline__ uint32_t fdiv(uint32_t e, uint32_t P, uint32_t mul) {
-  return P == 1 ? e : __umulhi(e, mul);
-}
-__host__ __device__ inline uint32_t fdiv_mul(uint32_t P) {
-  return P <= 1 ? 0u : (uint32_t)(((1ull << 32) + P - 1) / P);
-}
-
-constexpr int kGroups = 3;                    // loader groups (tiles round-robin)
-constexpr int kJB = 8;                        // 16 B channel pieces per pixel per load batch
-
-// One loader group (128 threads), thread = pixel.  Per tile a thread stages the dy pixel `gt`
-// and the x-halo pixels gt, gt+128, ...: one base address per pixel, then the pixel's channel
-// pieces are 16-byte loads at immediate offsets (no per-element index arithmetic), normalised
-// (BN affine from the shared-memory copy), rounded to TF32 and stored into the
-// SWIZZLE_128B_BASE32B tile layout (chunk = piece / 8, row = pixel, 16 B slot = piece % 8 XOR-ed
-// with the row's swizzle phase).
-__device__ __forceinline__ void wgrad_loader(const WgradTcParams& p, Ctl* ctl, uint32_t base,
-                                             const float4* s_aff, int grp, int gt, int t_begin,
-                                             int t_end, int ts, int co0, int ci0, int PD, int PX) {
-  const int lane = threadIdx.x & 31;
-  const bool stacked = p.taps_w > 1;
-  const int H = p.H, W = p.W, HP = p.HP;
-  const int tpi = p.tiles_w * p.tiles_h;
-  const uint32_t mulTpi = fdiv_mul(tpi), mulTw = fdiv_mul(p.tiles_w), mulT = fdiv_mul(p.TWp);
-  const uint32_t S = p.n_stages;
-  // a ring slot must have been consumed before a group can be two tiles ahead of it: with fewer
-  // slots than groups the third group sits out (parity aliasing otherwise)
-  const int n_groups = S >= (uint32_t)kGroups ? kGroups : 2;
-  if (grp >= n_groups) return;
-  // source split of the (possibly concatenated) x operand, in 16 B pieces of this channel block
-  const int c_split = p.S.nsrc > 1 ? p.S.s[0].C : (1 << 30);
-  const bool any_pool = p.S.s[0].pool || (p.S.nsrc > 1 && p.S.s[1].pool);
-  const bool has_aff = p.S.s[0].scale != nullptr || (p.S.nsrc > 1 && p.S.s[1].scale != nullptr);
-  // this thread's halo pixels (up to 5 slots of 128: dilated kernels), row/col within the halo
-  const uint32_t d_rel = p.x_bytes * (p.x3 ? 2 : 1) + (p.fs ? p.dpad * 1024 : 0);   // dy tile within a stage
-  const uint32_t d_row = d_rel + gt * 128, d_sw = (uint32_t)(gt & 3) << 5;
-  const int d_r = gt >> 3, d_c = gt & 7;
-  uint32_t st = grp % S, ph = ((grp / S) & 1) ^ 1;     // ring slot / empty-phase of this tile
-  const bool x3 = p.x3 != 0;
-  const uint32_t xlo_off = p.x_bytes, dlo_off = p.dy_bytes;    // hi tile -> lo tile (x3)
-  for (int tile = t_begin + grp * ts; tile < t_end; tile += n_groups * ts) {
-    const uint32_t x0 = base + st * p.stage_bytes;
-    const int n = (int)fdiv(tile, tpi, mulTpi);
-    const int rem = tile - n * tpi;
-    const int th_i = (int)fdiv(rem, p.tiles_w, mulTw);
-    const int tw_i = rem - th_i * p.tiles_w;
-    const int h0 = th_i * kTileH, w0 = tw_i * kTileW;
-    const int h_org = h0 - p.dil * (p.taps_h >> 1), w_org = w0 - p.dil * (p.taps_w >> 1);
-    const size_t img = (size_t)n * H;
-    mbar_wait(smem_u32(&ctl->empty[st]), ph);
-    // ---------------- x halo pixels
-    for (int q = gt; q < HP; q += kGroupThreads) {
-      const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-      const int gh = h_org + (int)hh, gw = w_org + (int)ww;
-      const bool ok = (unsigned)gh < (unsigned)H && (unsigned)gw < (unsigned)W;
-      const uint32_t row = x0 + q * 128, sw = (uint32_t)(q & 3) << 5;
-      if (!any_pool) {
-        const int ghc = min(max(gh, 0), H - 1), gwc = min(max(gw, 0), W - 1);
-        const size_t pixi = (img + ghc) * W + gwc;
-        const float* b0 = p.S.s[0].ptr + pixi * p.S.s[0].ld + ci0;
-        const float* b1 = p.S.nsrc > 1 ? p.S.s[1].ptr + pixi * p.S.s[1].ld + (ci0 - c_split) : b0;
-        const uint32_t msk = ok ? 0xFFFFFFFFu : 0u;
-        for (int jb = 0; jb < PX; jb += kJB) {
-          float4 v[kJB];
+// 4 consecutive channels (rows r0..r0+3) of pixel k: hi part, and the lo part at +lo_off (x3)
+__device__ __forceinline__ void put4(uint32_t base, int r0, int k, float4 v, bool x3, uint32_t lo_off) {
+  const float e[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-          for (int k = 0; k < kJB; ++k) {
-            const int j = jb + k;
-            if (j < PX) {
-              const float* src = (ci0 + j * 4 < c_split) ? b0 : b1;
-              v[k] = __ldg(reinterpret_cast<const float4*>(src + j * 4));
-            }
-          }
-#pragma unroll
-          for (int k = 0; k < kJB; ++k) {
-            const int j = jb + k;
-            if (j < PX) {
-              float4 x = v[k];
-              if (has_aff) {
-                const float4 sc = s_aff[2 * j], sh = s_aff[2 * j + 1];
-                x.x = fmaf(x.x, sc.x, sh.x); x.y = fmaf(x.y, sc.y, sh.y);
-                x.z = fmaf(x.z, sc.z, sh.z); x.w = fmaf(x.w, sc.w, sh.w);
-              }
-              const uint32_t dst = (stacked ? row : row + (j >> 3) * p.x_chunk) +
-                                   (((uint32_t)(j & 7) << 4) ^ sw);
-              sts128u(dst, tf32b(x.x) & msk, tf32b(x.y) & msk, tf32b(x.z) & msk, tf32b(x.w) & msk);
-              if (x3) {
-                const float4 l = part4(x, true);
-                sts128u(dst + xlo_off, tf32b(l.x) & msk, tf32b(l.y) & msk, tf32b(l.z) & msk,
-                        tf32b(l.w) & msk);
-              }
-            }
-          }
-        }
-      } else {
-        // pooled source(s): the generic normalise / max-pool / pad loader, piece by piece
-        for (int jb = 0; jb < PX; jb += 4) {
-          float4 v[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (jb + k < PX) v[k] = load_src4(p.S, n, gh, gw, H, W, ci0 + (jb + k) * 4);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int j = jb + k;
-            if (j < PX) {
-              const uint32_t dst = (stacked ? row : row + (j >> 3) * p.x_chunk) +
-                                   (((uint32_t)(j & 7) << 4) ^ sw);
-              sts128u(dst, tf32b(v[k].x), tf32b(v[k].y), tf32b(v[k].z), tf32b(v[k].w));
-              if (x3) {
-                const float4 l = part4(v[k], true);
-                sts128u(dst + xlo_off, tf32b(l.x), tf32b(l.y), tf32b(l.z), tf32b(l.w));
-              }
-            }
-          }
-        }
-      }
-    }
-    // ---------------- dy pixel gt of the 16 x 8 tile
-    {
-      const int gh = h0 + d_r, gw = w0 + d_c;
-      const bool ok = gh < H && gw < W;
-      const uint32_t msk = ok ? 0xFFFFFFFFu : 0u;
-      const float* db = p.dy + ((img + min(gh, H - 1)) * W + min(gw, W - 1)) * p.ld_dy + co0;
-      for (int jb = 0; jb < PD; jb += kJB) {
-        float4 v[kJB];
-#pragma unroll
-        for (int k = 0; k < kJB; ++k)
-          if (jb + k < PD) v[k] = __ldg(reinterpret_cast<const float4*>(db + (jb + k) * 4));
-#pragma unroll
-        for (int k = 0; k < kJB; ++k) {
-          const int j = jb + k;
-          if (j < PD) {
-            const uint32_t dst = x0 + d_row + (j >> 3) * kChunk + (((uint32_t)(j & 7) << 4) ^ d_sw);
-            sts128u(dst, tf32b(v[k].x) & msk, tf32b(v[k].y) & msk, tf32b(v[k].z) & msk,
-                    tf32b(v[k].w) & msk);
-            if (x3) {
-              const float4 l = part4(v[k], true);
-              sts128u(dst + dlo_off, tf32b(l.x) & msk, tf32b(l.y) & msk, tf32b(l.z) & msk,
-                      tf32b(l.w) & msk);
-            }
-          }
-        }
-      }
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&ctl->full[st]));
-    st += n_groups;
-    while (st >= S) { st -= S; ph ^= 1; }
+  for (int i = 0; i < 4; ++i) {
+    const uint32_t a = base + kmaj_off(r0 + i, k);
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(tf32b(e[i])) : "memory");
+    if (x3) asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + lo_off), "r"(tf32b(lo_part(e[i]))) : "memory");
   }
 }
 
-// Fast loader for un-pooled sources with <= 8 input pieces (one 32-channel block) and <= ND dy
-// pieces per pixel and a halo of <= 256 pixels: a thread owns the dy pixel `gt` and the halo
-// pixels gt and gt + 128, and issues EVERY load of the tile (up to 8 + 8 + ND float4) before it
-// waits for the shared-memory slot — one memory round trip per tile, overlapped with the MMAs of
-// the tiles in front of it, instead of three serialised ones behind the slot wait.
-template <int ND>
-__device__ __forceinline__ void wgrad_loader_fast(const WgradTcParams& p, Ctl* ctl, uint32_t base,
-                                                  const float4* s_aff, int grp, int gt, int t_begin,
-                                                  int t_end, int ts, int co0, int ci0, int PD, int PX) {
-  constexpr int NX = 8;
-  const int lane = threadIdx.x & 31;
-  const int H = p.H, W = p.W, HP = p.HP;
-  const int tpi = p.tiles_w * p.tiles_h;
-  const uint32_t mulTpi = fdiv_mul(tpi), mulTw = fdiv_mul(p.tiles_w), mulT = fdiv_mul(p.TWp);
-  const uint32_t S = p.n_stages;
-  const int n_groups = S >= (uint32_t)kGroups ? kGroups : 2;
-  if (grp >= n_groups) return;
-  const int c_split = p.S.nsrc > 1 ? p.S.s[0].C : (1 << 30);
-  const bool has_aff = p.S.s[0].scale != nullptr || (p.S.nsrc > 1 && p.S.s[1].scale != nullptr);
+template <int CIB>
+__global__ void __launch_bounds__(kThreads) wgrad_tc_kernel(const WgradTcParams p) {
+  constexpr int R = CIB / 2;
+  constexpr int QX = CIB / 4;                 // x quads per pixel
+  constexpr int ND = kPix * (kM / 4) / kThreads;   // dy float4 per thread per tile (8)
+  constexpr int NX = kPix * QX / kThreads;         // x float4 per thread per tile (2..8)
+  extern __shared__ __align__(128) uint8_t smem[];
+  const uint32_t sbase = smem_u32(smem);
+  const int tid = threadIdx.x;
+
+  // grid: x = pixel range, y = (tap, co block, ci block)
+  int blk = blockIdx.y;
+  const int cbi = blk % p.n_cib; blk /= p.n_cib;
+  const int cob = blk % p.n_cob; blk /= p.n_cob;
+  const int t = blk;
+  const int ty = t / p.taps_w, tx = t - ty * p.taps_w;
+  const int co0 = cob * kM, ci0 = cbi * CIB;
+  const int dh = (ty - (p.taps_h >> 1)) * p.dil, dwo = (tx - (p.taps_w >> 1)) * p.dil;
+  const int t_begin = (int)((int64_t)p.num_tiles * blockIdx.x / p.ranges);
+  const int t_end = (int)((int64_t)p.num_tiles * (blockIdx.x + 1) / p.ranges);
+  const int tpi = p.tiles_h * p.tiles_w;
   const bool x3 = p.x3 != 0;
-  const uint32_t xlo_off = p.x_bytes, dlo_off = p.dy_bytes;
-  const uint32_t d_rel = p.x_bytes * (p.x3 ? 2 : 1) + (p.fs ? p.dpad * 1024 : 0);
-  const uint32_t d_row = d_rel + gt * 128, d_sw = (uint32_t)(gt & 3) << 5;
-  const int d_r = gt >> 3, d_c = gt & 7;
-  const int q1 = gt + kGroupThreads;
-  const bool has_q1 = q1 < HP;
-  const uint32_t hh0 = fdiv(gt, p.TWp, mulT), ww0 = gt - hh0 * p.TWp;
-  const uint32_t hh1 = has_q1 ? fdiv(q1, p.TWp, mulT) : 0u, ww1 = has_q1 ? q1 - hh1 * p.TWp : 0u;
-  const uint32_t sw0 = (uint32_t)(gt & 3) << 5, sw1 = (uint32_t)(q1 & 3) << 5;
-  uint32_t st = grp % S, ph = ((grp / S) & 1) ^ 1;
-  for (int tile = t_begin + grp * ts; tile < t_end; tile += n_groups * ts) {
-    const uint32_t x0 = base + st * p.stage_bytes;
-    const int n = (int)fdiv(tile, tpi, mulTpi);
-    const int rem = tile - n * tpi;
-    const int th_i = (int)fdiv(rem, p.tiles_w, mulTw);
-    const int tw_i = rem - th_i * p.tiles_w;
-    const int h0 = th_i * kTileH, w0 = tw_i * kTileW;
-    const int h_org = h0 - p.dil * (p.taps_h >> 1), w_org = w0 - p.dil * (p.taps_w >> 1);
-    const size_t img = (size_t)n * H;
-    // ---- issue every load of this tile
-    float4 xa[NX], xb[NX], dv[ND];
-    const int gha = h_org + (int)hh0, gwa = w_org + (int)ww0;
-    const int ghb = h_org + (int)hh1, gwb = w_org + (int)ww1;
-    const bool oka = (unsigned)gha < (unsigned)H && (unsigned)gwa < (unsigned)W;
-    const bool okb = has_q1 && (unsigned)ghb < (unsigned)H && (unsigned)gwb < (unsigned)W;
-    {
-      const size_t pa = (img + min(max(gha, 0), H - 1)) * W + min(max(gwa, 0), W - 1);
-      const size_t pb = (img + min(max(ghb, 0), H - 1)) * W + min(max(gwb, 0), W - 1);
-      const float* a0 = p.S.s[0].ptr + pa * p.S.s[0].ld + ci0;
-      const float* a1 = p.S.nsrc > 1 ? p.S.s[1].ptr + pa * p.S.s[1].ld + (ci0 - c_split) : a0;
-      const float* b0 = p.S.s[0].ptr + pb * p.S.s[0].ld + ci0;
-      const float* b1 = p.S.nsrc > 1 ? p.S.s[1].ptr + pb * p.S.s[1].ld + (ci0 - c_split) : b0;
+  const int H = p.H, W = p.W;
+  const uint32_t a_lo = x3 ? (uint32_t)p.a_bytes : 0u;                     // dy_hi -> dy_lo
+  const uint32_t b_off = (uint32_t)p.a_bytes * (x3 ? 2 : 1);              // stage -> x_hi
+  const uint32_t b_lo = x3 ? (uint32_t)p.b_bytes : 0u;                     // x_hi -> x_lo
+
+  float4 dv[ND], xv[NX];
+  auto load = [&](int tile) {
+    const int n = tile / tpi, rem = tile - n * tpi;
+    const int h0 = (rem / p.tiles_w) * kTile, w0 = (rem % p.tiles_w) * kTile;
 #pragma unroll
-      for (int j = 0; j < NX; ++j)
-        if (j < PX) xa[j] = __ldg(reinterpret_cast<const float4*>(((ci0 + j * 4 < c_split) ? a0 : a1) + j * 4));
-      if (has_q1) {
-#pragma unroll
-        for (int j = 0; j < NX; ++j)
-          if (j < PX) xb[j] = __ldg(reinterpret_cast<const float4*>(((ci0 + j * 4 < c_split) ? b0 : b1) + j * 4));
-      }
+    for (int i = 0; i < ND; ++i) {
+      const int e = tid + kThreads * i;
+      const int k = (e >> 6) * 4 + (e & 3), q = (e >> 2) & 15;
+      const int gh = h0 + (k >> 3), gw = w0 + (k & 7), co = co0 + 4 * q;
+      dv[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (gh < H && gw < W && co < p.Cout)
+        dv[i] = __ldg(reinterpret_cast<const float4*>(p.dy + ((size_t)(n * H + gh) * W + gw) * p.ld_dy + co));
     }
-    const int ghd = h0 + d_r, gwd = w0 + d_c;
-    const bool okd = ghd < H && gwd < W;
-    {
-      const float* db = p.dy + ((img + min(ghd, H - 1)) * W + min(gwd, W - 1)) * p.ld_dy + co0;
 #pragma unroll
-      for (int j = 0; j < ND; ++j)
-        if (j < PD) dv[j] = __ldg(reinterpret_cast<const float4*>(db + j * 4));
+    for (int i = 0; i < NX; ++i) {
+      const int e = tid + kThreads * i;
+      const int k = (e / (4 * QX)) * 4 + (e & 3), q = (e >> 2) % QX;
+      const int ci = ci0 + 4 * q;
+      xv[i] = ci < p.Cin ? load_src4(p.S, n, h0 + (k >> 3) + dh, w0 + (k & 7) + dwo, H, W, ci)
+                         : make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    // ---- wait for the slot, transform, store
-    mbar_wait(smem_u32(&ctl->empty[st]), ph);
-    auto put_x = [&](float4 x, int j, uint32_t row, uint32_t sw, uint32_t msk) {
-      if (has_aff) {
-        const float4 sc = s_aff[2 * j], sh = s_aff[2 * j + 1];
-        x.x = fmaf(x.x, sc.x, sh.x); x.y = fmaf(x.y, sc.y, sh.y);
-        x.z = fmaf(x.z, sc.z, sh.z); x.w = fmaf(x.w, sc.w, sh.w);
-      }
-      const uint32_t dst = row + (((uint32_t)(j & 7) << 4) ^ sw);
-      sts128u(dst, tf32b(x.x) & msk, tf32b(x.y) & msk, tf32b(x.z) & msk, tf32b(x.w) & msk);
+  };
+  auto store = [&](uint32_t st) {
+#pragma unroll
+    for (int i = 0; i < ND; ++i) {
+      const int e = tid + kThreads * i;
+      put4(st, 4 * ((e >> 2) & 15), (e >> 6) * 4 + (e & 3), dv[i], x3, a_lo);
+    }
+#pragma unroll
+    for (int i = 0; i < NX; ++i) {
+      const int e = tid + kThreads * i;
+      put4(st + b_off, 4 * ((e >> 2) % QX), (e / (4 * QX)) * 4 + (e & 3), xv[i], x3, b_lo);
+    }
+  };
+
+  float acc[R];
+#pragma unroll
+  for (int i = 0; i < R; ++i) acc[i] = 0.f;
+  const uint64_t tmpl = wgmma_desc(0, 128, kSbo);
+  if (t_begin < t_end) load(t_begin);
+  int it = 0;
+  for (int tile = t_begin; tile < t_end; ++tile, ++it) {
+    const uint32_t st = sbase + (uint32_t)(it & 1) * p.stage_bytes;
+    store(st);
+    fence_proxy_async_smem();
+    __syncthreads();
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kPix / 8; ++ks) {
+      const uint32_t a = st + ks * 256, b = st + b_off + ks * 256;
+      Wgmma<CIB>::tf32(acc, tmpl | (a >> 4), tmpl | (b >> 4), 1u);
       if (x3) {
-        const float4 l = part4(x, true);
-        sts128u(dst + xlo_off, tf32b(l.x) & msk, tf32b(l.y) & msk, tf32b(l.z) & msk, tf32b(l.w) & msk);
-      }
-    };
-    {
-      const uint32_t ma = oka ? 0xFFFFFFFFu : 0u, mb = okb ? 0xFFFFFFFFu : 0u;
-#pragma unroll
-      for (int j = 0; j < NX; ++j)
-        if (j < PX) put_x(xa[j], j, x0 + gt * 128, sw0, ma);
-      if (has_q1) {
-#pragma unroll
-        for (int j = 0; j < NX; ++j)
-          if (j < PX) put_x(xb[j], j, x0 + q1 * 128, sw1, mb);
+        Wgmma<CIB>::tf32(acc, tmpl | ((a + a_lo) >> 4), tmpl | (b >> 4), 1u);
+        Wgmma<CIB>::tf32(acc, tmpl | (a >> 4), tmpl | ((b + b_lo) >> 4), 1u);
       }
     }
-    {
-      const uint32_t msk = okd ? 0xFFFFFFFFu : 0u;
-#pragma unroll
-      for (int j = 0; j < ND; ++j) {
-        if (j < PD) {
-          const uint32_t dst = x0 + d_row + (j >> 3) * kChunk + (((uint32_t)(j & 7) << 4) ^ d_sw);
-          sts128u(dst, tf32b(dv[j].x) & msk, tf32b(dv[j].y) & msk, tf32b(dv[j].z) & msk, tf32b(dv[j].w) & msk);
-          if (x3) {
-            const float4 l = part4(dv[j], true);
-            sts128u(dst + dlo_off, tf32b(l.x) & msk, tf32b(l.y) & msk, tf32b(l.z) & msk, tf32b(l.w) & msk);
-          }
-        }
-      }
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&ctl->full[st]));
-    st += n_groups;
-    while (st >= S) { st -= S; ph ^= 1; }
+    wgmma_commit();
+    if (tile + 1 < t_end) load(tile + 1);     // global loads in flight while the MMAs run
+    wgmma_wait<1>();                           // the group of tile - 1 (the other stage) retired
+    __syncthreads();
   }
-}
-
-// Element-mapped loader (round 2): consecutive lanes own consecutive 16-byte channel pieces of the
-// SAME pixel (PX / PD pieces per pixel, powers of two), so a warp's LDG.128 reads whole pixels
-// (coalesced 64-512 B runs) and its ST.SHARED.128 fills whole 128-byte swizzle rows (conflict
-// free) — the thread = pixel mapping of the loaders above touches 32 different lines per
-// instruction and measured 4200 warp instructions per tile (ncu, c6.0).  A thread's piece index
-// and therefore its source tensor, its BatchNorm scale/shift (registers, not shared memory) and
-// its swizzle phase are loop constants; per element there is one address multiply-add, the
-// affine, the TF32 rounding add and one store.  Pooled sources (2x2 max of the affine'd window)
-// take four loads per element in the same mapping.  XB = elements in flight per thread.
-template <int XB>
-__device__ __forceinline__ void wgrad_loader_elem(const WgradTcParams& p, Ctl* ctl, uint32_t base,
-                                                  int grp, int gt, int t_begin, int t_end, int ts,
-                                                  int co0, int ci0, int PD, int PX) {
-  const int lane = threadIdx.x & 31;
-  const bool stacked = p.taps_w > 1;
-  const int H = p.H, W = p.W, HP = p.HP;
-  const int tpi = p.tiles_w * p.tiles_h;
-  const uint32_t mulTpi = fdiv_mul(tpi), mulTw = fdiv_mul(p.tiles_w), mulT = fdiv_mul(p.TWp);
-  const uint32_t S = p.n_stages;
-  const int n_groups = S >= (uint32_t)kGroups ? kGroups : 2;
-  if (grp >= n_groups) return;
-  const bool x3 = p.x3 != 0;
-  const uint32_t xlo_off = p.x_bytes, dlo_off = p.dy_bytes;
-  // ---- x operand: piece j of halo pixels q0, q0 + QS, ...
-  const int j = gt & (PX - 1);
-  const int lx = 31 - __clz(PX);                       // log2(PX)
-  const int QS = kGroupThreads >> lx, q0 = gt >> lx;
-  const int ux_total = (HP + QS - 1 - q0) / QS;          // this thread's halo pixels: q0 + u*QS < HP
-  int cx = ci0 + j * 4;
-  const SrcDev* sp = &p.S.s[0];
-  if (p.S.nsrc > 1 && cx >= p.S.s[0].C) { sp = &p.S.s[1]; cx -= p.S.s[0].C; }
-  const bool has_aff = sp->scale != nullptr, pool = sp->pool != 0;
-  const int up_mode = sp->pool >= AB_SRC_UP_BILINEAR ? sp->pool : 0;
-  float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (has_aff) {
-    sc = __ldg(reinterpret_cast<const float4*>(sp->scale + cx));
-    sh = __ldg(reinterpret_cast<const float4*>(sp->shift + cx));
-  }
-  const float* xsrc = sp->ptr + cx;
-  const uint32_t xld = sp->ld;
-  // (q & 3) is the same for all of a thread's pixels: QS is a multiple of 4
-  const uint32_t x_dst0 = (uint32_t)q0 * 128 + (stacked ? 0u : (uint32_t)(j >> 3) * p.x_chunk) +
-                          (((uint32_t)(j & 7) << 4) ^ ((uint32_t)(q0 & 3) << 5));
-  const uint32_t x_step = (uint32_t)QS * 128;
-  // ---- dy operand: piece jd of tile pixels pd0, pd0 + QD, ...
-  const int jd = gt & (PD - 1);
-  const int ld_ = 31 - __clz(PD);
-  const int QD = kGroupThreads >> ld_, pd0 = gt >> ld_;
-  const uint32_t d_rel = p.x_bytes * (p.x3 ? 2 : 1) + (p.fs ? p.dpad * 1024 : 0);
-  const uint32_t d_dst0 = d_rel + (uint32_t)pd0 * 128 + (uint32_t)(jd >> 3) * kChunk +
-                          (((uint32_t)(jd & 7) << 4) ^ ((uint32_t)(pd0 & 3) << 5));
-  const uint32_t d_step = (uint32_t)QD * 128;
-  const float* dsrc = p.dy + co0 + jd * 4;
-  uint32_t st = grp % S, ph = ((grp / S) & 1) ^ 1;
-  for (int tile = t_begin + grp * ts; tile < t_end; tile += n_groups * ts) {
-    const uint32_t x0 = base + st * p.stage_bytes;
-    const int n = (int)fdiv(tile, tpi, mulTpi);
-    const int rem = tile - n * tpi;
-    const int th_i = (int)fdiv(rem, p.tiles_w, mulTw);
-    const int tw_i = rem - th_i * p.tiles_w;
-    const int h0 = th_i * kTileH, w0 = tw_i * kTileW;
-    const int h_org = h0 - p.dil * (p.taps_h >> 1), w_org = w0 - p.dil * (p.taps_w >> 1);
-    const bool interior = h_org >= 0 && w_org >= 0 && h_org + p.THp <= H && w_org + p.TWp <= W;
-    bool waited = false;
-    if (p.l2_prefetch) {
-      // experiment, default off: pull the group's NEXT tile into L2 (one request per 32-byte sector)
-      const int nt = tile + n_groups * ts;
-      if (nt < t_end && !(j & 1)) {
-        const int n2 = (int)fdiv(nt, tpi, mulTpi);
-        const int rem2 = nt - n2 * tpi;
-        const int th2 = (int)fdiv(rem2, p.tiles_w, mulTw);
-        const int tw2 = rem2 - th2 * p.tiles_w;
-        const int ho2 = th2 * kTileH - p.dil * (p.taps_h >> 1), wo2 = tw2 * kTileW - p.dil * (p.taps_w >> 1);
-        if (!pool) {
-          for (int u = 0; u < ux_total; ++u) {
-            const uint32_t q = (uint32_t)(q0 + u * QS);
-            const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-            const int ghc = min(max(ho2 + (int)hh, 0), H - 1), gwc = min(max(wo2 + (int)ww, 0), W - 1);
-            prefetch_l2(xsrc + ((size_t)(n2 * H + ghc) * W + gwc) * xld);
-          }
-        }
-      }
-      if (nt < t_end && !(jd & 1)) {
-        const int n2 = (int)fdiv(nt, tpi, mulTpi);
-        const int rem2 = nt - n2 * tpi;
-        const int th2 = (int)fdiv(rem2, p.tiles_w, mulTw);
-        const int tw2 = rem2 - th2 * p.tiles_w;
-        for (int u = 0; u < PD; ++u) {
-          const int pd = pd0 + u * QD;
-          const int gh = min(th2 * kTileH + (pd >> 3), H - 1), gw = min(tw2 * kTileW + (pd & 7), W - 1);
-          prefetch_l2(dsrc + ((size_t)(n2 * H + gh) * W + gw) * p.ld_dy);
-        }
-      }
-    }
-    // ---------------- x halo elements, XB at a time
-    for (int ub = 0; ub < ux_total; ub += XB) {
-      float4 v[XB];
-      uint32_t okm = 0;
-      if (!pool) {
-        const float* tb = xsrc + ((size_t)(n * H + h_org) * W + w_org) * xld;   // interior tiles only
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  // this CTA's partial D[64][CIB] (row-major) into its slot; the last range of the group adds the
+  // ranges in order into dW
+  const int warp = tid >> 5, lane = tid & 31;
+  const int taps = p.taps_h * p.taps_w;
+  constexpr int n = kM * CIB;
+  double* slot = ordered_slot(p.red, blockIdx.y, gridDim.x, blockIdx.x, n);
 #pragma unroll
-        for (int k = 0; k < XB; ++k) {
-          const int u = ub + k;
-          if (u < ux_total) {
-            const uint32_t q = (uint32_t)(q0 + u * QS);
-            const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-            if (interior) {
-              v[k] = __ldg(reinterpret_cast<const float4*>(tb + (size_t)(hh * W + ww) * xld));
-              okm |= 1u << k;
-            } else {
-              const int gh = h_org + (int)hh, gw = w_org + (int)ww;
-              const bool ok = (unsigned)gh < (unsigned)H && (unsigned)gw < (unsigned)W;
-              const int ghc = min(max(gh, 0), H - 1), gwc = min(max(gw, 0), W - 1);
-              v[k] = __ldg(reinterpret_cast<const float4*>(xsrc + ((size_t)(n * H + ghc) * W + gwc) * xld));
-              okm |= (ok ? 1u : 0u) << k;
-            }
-          }
-        }
+  for (int j = 0; j < R / 4; ++j)
 #pragma unroll
-        for (int k = 0; k < XB; ++k) {
-          const bool ok = (okm >> k) & 1u;
-          v[k].x = ok ? fmaf(v[k].x, sc.x, sh.x) : 0.f;
-          v[k].y = ok ? fmaf(v[k].y, sc.y, sh.y) : 0.f;
-          v[k].z = ok ? fmaf(v[k].z, sc.z, sh.z) : 0.f;
-          v[k].w = ok ? fmaf(v[k].w, sc.w, sh.w) : 0.f;
-        }
-      } else if (up_mode) {
-        // 2x upsampling on load: this piece belongs to the decoder's (H/2, W/2) source
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int k = 0; k < XB; ++k) {
-          const int u = ub + k;
-          v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (u < ux_total) {
-            const uint32_t q = (uint32_t)(q0 + u * QS);
-            const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-            const int gh = h_org + (int)hh, gw = w_org + (int)ww;
-            const bool ok = (unsigned)gh < (unsigned)H && (unsigned)gw < (unsigned)W;
-            const float4 a = load_up4(xsrc, (int)xld, up_mode, n, min(max(gh, 0), H - 1),
-                                      min(max(gw, 0), W - 1), H, W);
-            if (ok)
-              v[k] = make_float4(fmaf(a.x, sc.x, sh.x), fmaf(a.y, sc.y, sh.y), fmaf(a.z, sc.z, sh.z),
-                                 fmaf(a.w, sc.w, sh.w));
-            okm |= 1u << k;
-          }
-        }
-      } else {
-        const int H2 = 2 * H, W2 = 2 * W;
-        const size_t rs = (size_t)W2 * xld;
-#pragma unroll
-        for (int k = 0; k < XB; ++k) {
-          const int u = ub + k;
-          v[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (u < ux_total) {
-            const uint32_t q = (uint32_t)(q0 + u * QS);
-            const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-            const int gh = h_org + (int)hh, gw = w_org + (int)ww;
-            const bool ok = (unsigned)gh < (unsigned)H && (unsigned)gw < (unsigned)W;
-            const int ghc = min(max(gh, 0), H - 1), gwc = min(max(gw, 0), W - 1);
-            const float* q0p = xsrc + ((size_t)(n * H2 + 2 * ghc) * W2 + 2 * gwc) * xld;
-            const float4 a0 = __ldg(reinterpret_cast<const float4*>(q0p));
-            const float4 a1 = __ldg(reinterpret_cast<const float4*>(q0p + xld));
-            const float4 a2 = __ldg(reinterpret_cast<const float4*>(q0p + rs));
-            const float4 a3 = __ldg(reinterpret_cast<const float4*>(q0p + rs + xld));
-            if (ok) {
-              v[k].x = fmaxf(fmaxf(fmaf(a0.x, sc.x, sh.x), fmaf(a1.x, sc.x, sh.x)),
-                             fmaxf(fmaf(a2.x, sc.x, sh.x), fmaf(a3.x, sc.x, sh.x)));
-              v[k].y = fmaxf(fmaxf(fmaf(a0.y, sc.y, sh.y), fmaf(a1.y, sc.y, sh.y)),
-                             fmaxf(fmaf(a2.y, sc.y, sh.y), fmaf(a3.y, sc.y, sh.y)));
-              v[k].z = fmaxf(fmaxf(fmaf(a0.z, sc.z, sh.z), fmaf(a1.z, sc.z, sh.z)),
-                             fmaxf(fmaf(a2.z, sc.z, sh.z), fmaf(a3.z, sc.z, sh.z)));
-              v[k].w = fmaxf(fmaxf(fmaf(a0.w, sc.w, sh.w), fmaf(a1.w, sc.w, sh.w)),
-                             fmaxf(fmaf(a2.w, sc.w, sh.w), fmaf(a3.w, sc.w, sh.w)));
-            }
-            okm |= 1u << k;
-          }
-        }
-      }
-      if (!waited) {
-        mbar_wait(smem_u32(&ctl->empty[st]), ph);
-        waited = true;
-      }
-#pragma unroll
-      for (int k = 0; k < XB; ++k) {
-        const int u = ub + k;
-        if (u < ux_total) {
-          const uint32_t dst = x0 + x_dst0 + (uint32_t)u * x_step;
-          sts128u(dst, tf32b(v[k].x), tf32b(v[k].y), tf32b(v[k].z), tf32b(v[k].w));
-          if (x3) {
-            const float4 l = part4(v[k], true);
-            sts128u(dst + xlo_off, tf32b(l.x), tf32b(l.y), tf32b(l.z), tf32b(l.w));
-          }
-        }
-      }
-    }
-    // ---------------- dy elements (PD per thread), 8 at a time
-    {
-      const size_t img = (size_t)n * H;
-      for (int ub = 0; ub < PD; ub += 8) {
-        float4 v[8];
-        uint32_t okm = 0;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int u = ub + k;
-          if (u < PD) {
-            const int pd = pd0 + u * QD;
-            const int gh = h0 + (pd >> 3), gw = w0 + (pd & 7);
-            const bool ok = gh < H && gw < W;
-            v[k] = __ldg(reinterpret_cast<const float4*>(
-                dsrc + ((img + min(gh, H - 1)) * W + min(gw, W - 1)) * p.ld_dy));
-            okm |= (ok ? 1u : 0u) << k;
-          }
-        }
-        if (!waited) {
-          mbar_wait(smem_u32(&ctl->empty[st]), ph);
-          waited = true;
-        }
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int u = ub + k;
-          if (u < PD) {
-            const uint32_t msk = ((okm >> k) & 1u) ? 0xFFFFFFFFu : 0u;
-            const uint32_t dst = x0 + d_dst0 + (uint32_t)u * d_step;
-            sts128u(dst, tf32b(v[k].x) & msk, tf32b(v[k].y) & msk, tf32b(v[k].z) & msk, tf32b(v[k].w) & msk);
-            if (x3) {
-              const float4 l = part4(v[k], true);
-              sts128u(dst + dlo_off, tf32b(l.x) & msk, tf32b(l.y) & msk, tf32b(l.z) & msk, tf32b(l.w) & msk);
-            }
-          }
-        }
-      }
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&ctl->full[st]));
-    st += n_groups;
-    while (st >= S) { st -= S; ph ^= 1; }
-  }
-}
-
-// Compile-time specialisation of the element-mapped loader for un-pooled sources (ncu source view
-// of the run-time version on c6.0: 1260 warp instructions per tile and warp, 79 per 16-byte
-// element — per-element validity branches with their BSYNCs, the halo index arithmetic and
-// constant-bank reloads).  UX = halo elements per thread (only the LAST one can be absent:
-// HP is not a multiple of the pixel stride QS), UD = dy elements per thread, X3 = split operands.
-// The halo offsets of a thread's elements are loop constants held in registers, the affine is
-// applied unconditionally (scale 1 / shift 0 without BatchNorm), interior tiles take a path
-// without clamps or masks.
-template <int UX, int UD, bool X3>
-__device__ __forceinline__ void wgrad_loader_ct(const WgradTcParams& p, Ctl* ctl, uint32_t base,
-                                                int grp, int gt, int t_begin, int t_end, int ts,
-                                                int co0, int ci0, int PX) {
-  constexpr int PD = UD;
-  const int lane = threadIdx.x & 31;
-  const bool stacked = p.taps_w > 1;
-  const int H = p.H, W = p.W, HP = p.HP;
-  const int tpi = p.tiles_w * p.tiles_h;
-  const uint32_t mulTpi = fdiv_mul(tpi), mulTw = fdiv_mul(p.tiles_w), mulT = fdiv_mul(p.TWp);
-  const uint32_t S = p.n_stages;
-  const int n_groups = S >= (uint32_t)kGroups ? kGroups : 2;
-  if (grp >= n_groups) return;
-  const uint32_t xlo_off = p.x_bytes, dlo_off = p.dy_bytes;
-  const int j = gt & (PX - 1);
-  const int lx = 31 - __clz(PX);
-  const int QS = kGroupThreads >> lx, q0 = gt >> lx;
-  int cx = ci0 + j * 4;
-  const SrcDev* sp = &p.S.s[0];
-  if (p.S.nsrc > 1 && cx >= p.S.s[0].C) { sp = &p.S.s[1]; cx -= p.S.s[0].C; }
-  float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (sp->scale != nullptr) {
-    sc = __ldg(reinterpret_cast<const float4*>(sp->scale + cx));
-    sh = __ldg(reinterpret_cast<const float4*>(sp->shift + cx));
-  }
-  const float* xsrc = sp->ptr + cx;
-  const uint32_t xld = sp->ld;
-  uint32_t pix[UX];
-#pragma unroll
-  for (int u = 0; u < UX; ++u) {
-    const uint32_t q = min((uint32_t)(q0 + u * QS), (uint32_t)(HP - 1));
-    const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-    pix[u] = (hh * (uint32_t)W + ww) * xld;
-  }
-  const bool last_valid = q0 + (UX - 1) * QS < HP;
-  const uint32_t x_dst0 = (uint32_t)q0 * 128 + (stacked ? 0u : (uint32_t)(j >> 3) * p.x_chunk) +
-                          (((uint32_t)(j & 7) << 4) ^ ((uint32_t)(q0 & 3) << 5));
-  const uint32_t x_step = (uint32_t)QS * 128;
-  constexpr int ld_ = UD == 4 ? 2 : (UD == 8 ? 3 : (UD == 16 ? 4 : 5));
-  const int jd = gt & (PD - 1);
-  constexpr int QD = kGroupThreads >> ld_;
-  const int pd0 = gt >> ld_;
-  const uint32_t d_rel = p.x_bytes * (X3 ? 2 : 1) + (p.fs ? p.dpad * 1024 : 0);
-  const uint32_t d_dst0 = d_rel + (uint32_t)pd0 * 128 + (uint32_t)(jd >> 3) * kChunk +
-                          (((uint32_t)(jd & 7) << 4) ^ ((uint32_t)(pd0 & 3) << 5));
-  constexpr uint32_t d_step = (uint32_t)QD * 128;
-  const float* dsrc = p.dy + co0 + jd * 4;
-  const uint32_t dld = p.ld_dy;
-  uint32_t st = grp % S, ph = ((grp / S) & 1) ^ 1;
-  for (int tile = t_begin + grp * ts; tile < t_end; tile += n_groups * ts) {
-    const uint32_t x0 = base + st * p.stage_bytes;
-    const int n = (int)fdiv(tile, tpi, mulTpi);
-    const int rem = tile - n * tpi;
-    const int th_i = (int)fdiv(rem, p.tiles_w, mulTw);
-    const int tw_i = rem - th_i * p.tiles_w;
-    const int h0 = th_i * kTileH, w0 = tw_i * kTileW;
-    const int h_org = h0 - p.dil * (p.taps_h >> 1), w_org = w0 - p.dil * (p.taps_w >> 1);
-    const bool interior = h_org >= 0 && w_org >= 0 && h_org + p.THp <= H && w_org + p.TWp <= W;
-    const bool dfull = h0 + kTileH <= H && w0 + kTileW <= W;
-    float4 v[UX];
-    if (interior) {
-      const float* tb = xsrc + ((size_t)(n * H + h_org) * W + w_org) * xld;
-#pragma unroll
-      for (int u = 0; u < UX; ++u) {
-        if (u < UX - 1 || last_valid) v[u] = __ldg(reinterpret_cast<const float4*>(tb + pix[u]));
-      }
-#pragma unroll
-      for (int u = 0; u < UX; ++u) {
-        v[u].x = fmaf(v[u].x, sc.x, sh.x); v[u].y = fmaf(v[u].y, sc.y, sh.y);
-        v[u].z = fmaf(v[u].z, sc.z, sh.z); v[u].w = fmaf(v[u].w, sc.w, sh.w);
-      }
-    } else {
-      uint32_t okm = 0;
-#pragma unroll
-      for (int u = 0; u < UX; ++u) {
-        const uint32_t q = min((uint32_t)(q0 + u * QS), (uint32_t)(HP - 1));   // border tiles: recompute
-        const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-        const int gh = h_org + (int)hh, gw = w_org + (int)ww;
-        const bool ok = (unsigned)gh < (unsigned)H && (unsigned)gw < (unsigned)W;
-        const int ghc = min(max(gh, 0), H - 1), gwc = min(max(gw, 0), W - 1);
-        if (u < UX - 1 || last_valid)
-          v[u] = __ldg(reinterpret_cast<const float4*>(xsrc + ((size_t)(n * H + ghc) * W + gwc) * xld));
-        okm |= (ok ? 1u : 0u) << u;
-      }
-#pragma unroll
-      for (int u = 0; u < UX; ++u) {
-        const bool ok = (okm >> u) & 1u;
-        v[u].x = ok ? fmaf(v[u].x, sc.x, sh.x) : 0.f; v[u].y = ok ? fmaf(v[u].y, sc.y, sh.y) : 0.f;
-        v[u].z = ok ? fmaf(v[u].z, sc.z, sh.z) : 0.f; v[u].w = ok ? fmaf(v[u].w, sc.w, sh.w) : 0.f;
-      }
-    }
-    // first batch of dy elements rides along with the x loads
-    constexpr int DB = 4;
-    float4 dv[DB];
-    uint32_t dokm = 0;
-    auto load_dy = [&](int ub) {
-      dokm = 0;
-      const size_t img = (size_t)n * H;
-#pragma unroll
-      for (int k = 0; k < DB; ++k) {
-        const int pd = pd0 + (ub + k) * QD;
-        const int gh = h0 + (pd >> 3), gw = w0 + (pd & 7);
-        if (dfull) {
-          dv[k] = __ldg(reinterpret_cast<const float4*>(dsrc + ((img + gh) * W + gw) * dld));
-          dokm |= 1u << k;
-        } else {
-          const bool ok = gh < H && gw < W;
-          dv[k] = __ldg(reinterpret_cast<const float4*>(dsrc + ((img + min(gh, H - 1)) * W + min(gw, W - 1)) * dld));
-          dokm |= (ok ? 1u : 0u) << k;
-        }
-      }
-    };
-    auto store_dy = [&](int ub) {
-#pragma unroll
-      for (int k = 0; k < DB; ++k) {
-        const uint32_t msk = ((dokm >> k) & 1u) ? 0xFFFFFFFFu : 0u;
-        const uint32_t dst = x0 + d_dst0 + (uint32_t)(ub + k) * d_step;
-        sts128u(dst, tf32b(dv[k].x) & msk, tf32b(dv[k].y) & msk, tf32b(dv[k].z) & msk, tf32b(dv[k].w) & msk);
-        if (X3) {
-          const float4 l = part4(dv[k], true);
-          sts128u(dst + dlo_off, tf32b(l.x) & msk, tf32b(l.y) & msk, tf32b(l.z) & msk, tf32b(l.w) & msk);
-        }
-      }
-    };
-    load_dy(0);
-    mbar_wait(smem_u32(&ctl->empty[st]), ph);
-#pragma unroll
-    for (int u = 0; u < UX; ++u) {
-      if (u < UX - 1 || last_valid) {
-        const uint32_t dst = x0 + x_dst0 + (uint32_t)u * x_step;
-        sts128u(dst, tf32b(v[u].x), tf32b(v[u].y), tf32b(v[u].z), tf32b(v[u].w));
-        if (X3) {
-          const float4 l = part4(v[u], true);
-          sts128u(dst + xlo_off, tf32b(l.x), tf32b(l.y), tf32b(l.z), tf32b(l.w));
-        }
-      }
-    }
-    store_dy(0);
-#pragma unroll
-    for (int ub = DB; ub < UD; ub += DB) {
-      load_dy(ub);
-      store_dy(ub);
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&ctl->full[st]));
-    st += n_groups;
-    while (st >= S) { st -= S; ph ^= 1; }
-  }
-}
-
-// Batched variant of wgrad_loader_ct for the shapes whose elements do not fit the register file
-// at once: pooled sources (four loads per element: 2x2 max of the affine'd window) and the 1x1
-// layers with 128 input channels per CTA (32 elements per thread).  XB elements are in flight;
-// halo offsets are recomputed per element (4 integer instructions), everything else as above.
-template <int UX, int XB, int UD, bool POOL>
-__device__ __forceinline__ void wgrad_loader_ctb(const WgradTcParams& p, Ctl* ctl, uint32_t base,
-                                                 int grp, int gt, int t_begin, int t_end, int ts,
-                                                 int co0, int ci0, int PX) {
-  constexpr int PD = UD;
-  const int lane = threadIdx.x & 31;
-  const bool stacked = p.taps_w > 1;
-  const int H = p.H, W = p.W, HP = p.HP;
-  const int tpi = p.tiles_w * p.tiles_h;
-  const uint32_t mulTpi = fdiv_mul(tpi), mulTw = fdiv_mul(p.tiles_w), mulT = fdiv_mul(p.TWp);
-  const uint32_t S = p.n_stages;
-  const int n_groups = S >= (uint32_t)kGroups ? kGroups : 2;
-  if (grp >= n_groups) return;
-  const int j = gt & (PX - 1);
-  const int lx = 31 - __clz(PX);
-  const int QS = kGroupThreads >> lx, q0 = gt >> lx;
-  int cx = ci0 + j * 4;
-  const SrcDev* sp = &p.S.s[0];
-  if (p.S.nsrc > 1 && cx >= p.S.s[0].C) { sp = &p.S.s[1]; cx -= p.S.s[0].C; }
-  float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (sp->scale != nullptr) {
-    sc = __ldg(reinterpret_cast<const float4*>(sp->scale + cx));
-    sh = __ldg(reinterpret_cast<const float4*>(sp->shift + cx));
-  }
-  const float* xsrc = sp->ptr + cx;
-  const uint32_t xld = sp->ld;
-  const bool last_valid = q0 + (UX - 1) * QS < HP;
-  const uint32_t x_dst0 = (uint32_t)q0 * 128 + (stacked ? 0u : (uint32_t)(j >> 3) * p.x_chunk) +
-                          (((uint32_t)(j & 7) << 4) ^ ((uint32_t)(q0 & 3) << 5));
-  const uint32_t x_step = (uint32_t)QS * 128;
-  constexpr int ld_ = UD == 4 ? 2 : (UD == 8 ? 3 : (UD == 16 ? 4 : 5));
-  const int jd = gt & (PD - 1);
-  constexpr int QD = kGroupThreads >> ld_;
-  const int pd0 = gt >> ld_;
-  const uint32_t d_rel = p.x_bytes + (p.fs ? p.dpad * 1024 : 0);
-  const uint32_t d_dst0 = d_rel + (uint32_t)pd0 * 128 + (uint32_t)(jd >> 3) * kChunk +
-                          (((uint32_t)(jd & 7) << 4) ^ ((uint32_t)(pd0 & 3) << 5));
-  constexpr uint32_t d_step = (uint32_t)QD * 128;
-  const float* dsrc = p.dy + co0 + jd * 4;
-  const uint32_t dld = p.ld_dy;
-  const int Hs = POOL ? 2 * H : H, Ws = POOL ? 2 * W : W;       // source extent
-  const size_t rs = (size_t)Ws * xld;
-  uint32_t st = grp % S, ph = ((grp / S) & 1) ^ 1;
-  for (int tile = t_begin + grp * ts; tile < t_end; tile += n_groups * ts) {
-    const uint32_t x0 = base + st * p.stage_bytes;
-    const int n = (int)fdiv(tile, tpi, mulTpi);
-    const int rem = tile - n * tpi;
-    const int th_i = (int)fdiv(rem, p.tiles_w, mulTw);
-    const int tw_i = rem - th_i * p.tiles_w;
-    const int h0 = th_i * kTileH, w0 = tw_i * kTileW;
-    const int h_org = h0 - p.dil * (p.taps_h >> 1), w_org = w0 - p.dil * (p.taps_w >> 1);
-    const bool interior = h_org >= 0 && w_org >= 0 && h_org + p.THp <= H && w_org + p.TWp <= W;
-    const bool dfull = h0 + kTileH <= H && w0 + kTileW <= W;
-    const float* img = xsrc + (size_t)n * Hs * rs;
-    constexpr int DB = 4;
-    float4 dv[DB];
-    uint32_t dokm = 0;
-    auto load_dy = [&](int ub) {
-      dokm = 0;
-      const size_t im = (size_t)n * H;
-#pragma unroll
-      for (int k = 0; k < DB; ++k) {
-        const int pd = pd0 + (ub + k) * QD;
-        const int gh = h0 + (pd >> 3), gw = w0 + (pd & 7);
-        const bool ok = dfull || (gh < H && gw < W);
-        dv[k] = __ldg(reinterpret_cast<const float4*>(dsrc + ((im + min(gh, H - 1)) * W + min(gw, W - 1)) * dld));
-        dokm |= (ok ? 1u : 0u) << k;
-      }
-    };
-    auto store_dy = [&](int ub) {
-#pragma unroll
-      for (int k = 0; k < DB; ++k) {
-        const uint32_t msk = ((dokm >> k) & 1u) ? 0xFFFFFFFFu : 0u;
-        sts128u(x0 + d_dst0 + (uint32_t)(ub + k) * d_step, tf32b(dv[k].x) & msk, tf32b(dv[k].y) & msk,
-                tf32b(dv[k].z) & msk, tf32b(dv[k].w) & msk);
-      }
-    };
-#pragma unroll
-    for (int ub = 0; ub < UX; ub += XB) {
-      float4 v[XB];
-      uint32_t okm = 0;
-#pragma unroll
-      for (int k = 0; k < XB; ++k) {
-        const int u = ub + k;
-        if (u < UX && (u < UX - 1 || last_valid)) {
-          const uint32_t q = (uint32_t)(q0 + u * QS);
-          const uint32_t hh = fdiv(q, p.TWp, mulT), ww = q - hh * p.TWp;
-          const int gh = h_org + (int)hh, gw = w_org + (int)ww;
-          const bool ok = interior || ((unsigned)gh < (unsigned)H && (unsigned)gw < (unsigned)W);
-          const int ghc = interior ? gh : min(max(gh, 0), H - 1);
-          const int gwc = interior ? gw : min(max(gw, 0), W - 1);
-          okm |= (ok ? 1u : 0u) << k;
-          if (!POOL) {
-            v[k] = __ldg(reinterpret_cast<const float4*>(img + (size_t)ghc * rs + (size_t)gwc * xld));
-          } else {
-            const float* q0p = img + (size_t)(2 * ghc) * rs + (size_t)(2 * gwc) * xld;
-            const float4 a0 = __ldg(reinterpret_cast<const float4*>(q0p));
-            const float4 a1 = __ldg(reinterpret_cast<const float4*>(q0p + xld));
-            const float4 a2 = __ldg(reinterpret_cast<const float4*>(q0p + rs));
-            const float4 a3 = __ldg(reinterpret_cast<const float4*>(q0p + rs + xld));
-            // affine BEFORE the max (a negative BatchNorm scale flips the order)
-            v[k].x = fmaxf(fmaxf(fmaf(a0.x, sc.x, sh.x), fmaf(a1.x, sc.x, sh.x)),
-                           fmaxf(fmaf(a2.x, sc.x, sh.x), fmaf(a3.x, sc.x, sh.x)));
-            v[k].y = fmaxf(fmaxf(fmaf(a0.y, sc.y, sh.y), fmaf(a1.y, sc.y, sh.y)),
-                           fmaxf(fmaf(a2.y, sc.y, sh.y), fmaf(a3.y, sc.y, sh.y)));
-            v[k].z = fmaxf(fmaxf(fmaf(a0.z, sc.z, sh.z), fmaf(a1.z, sc.z, sh.z)),
-                           fmaxf(fmaf(a2.z, sc.z, sh.z), fmaf(a3.z, sc.z, sh.z)));
-            v[k].w = fmaxf(fmaxf(fmaf(a0.w, sc.w, sh.w), fmaf(a1.w, sc.w, sh.w)),
-                           fmaxf(fmaf(a2.w, sc.w, sh.w), fmaf(a3.w, sc.w, sh.w)));
-          }
-        }
-      }
-      if (ub == 0) {
-        load_dy(0);
-        mbar_wait(smem_u32(&ctl->empty[st]), ph);
-      }
-#pragma unroll
-      for (int k = 0; k < XB; ++k) {
-        const int u = ub + k;
-        if (u < UX && (u < UX - 1 || last_valid)) {
-          const bool ok = (okm >> k) & 1u;
-          float4 r = v[k];
-          if (!POOL) {
-            r.x = fmaf(r.x, sc.x, sh.x); r.y = fmaf(r.y, sc.y, sh.y);
-            r.z = fmaf(r.z, sc.z, sh.z); r.w = fmaf(r.w, sc.w, sh.w);
-          }
-          const uint32_t m = ok ? 0xFFFFFFFFu : 0u;
-          sts128u(x0 + x_dst0 + (uint32_t)u * x_step, tf32b(r.x) & m, tf32b(r.y) & m, tf32b(r.z) & m,
-                  tf32b(r.w) & m);
-        }
-      }
-      if (ub == 0) store_dy(0);
-    }
-#pragma unroll
-    for (int ub = DB; ub < UD; ub += DB) {
-      load_dy(ub);
-      store_dy(ub);
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(smem_u32(&ctl->full[st]));
-    st += n_groups;
-    while (st >= S) { st -= S; ph ^= 1; }
-  }
-}
-
-template <int UX, int XB, bool POOL>
-__device__ __forceinline__ void wgrad_loader_ctb_ud(const WgradTcParams& p, Ctl* ctl, uint32_t base,
-                                                    int grp, int gt, int t_begin, int t_end, int ts,
-                                                    int co0, int ci0, int PD, int PX) {
-  if (PD == 4) wgrad_loader_ctb<UX, XB, 4, POOL>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-  else if (PD == 8) wgrad_loader_ctb<UX, XB, 8, POOL>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-  else if (PD == 16) wgrad_loader_ctb<UX, XB, 16, POOL>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-  else wgrad_loader_ctb<UX, XB, 32, POOL>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-}
-
-template <int UX, bool X3>
-__device__ __forceinline__ void wgrad_loader_ct_ud(const WgradTcParams& p, Ctl* ctl, uint32_t base,
-                                                   int grp, int gt, int t_begin, int t_end, int ts,
-                                                   int co0, int ci0, int PD, int PX) {
-  if (PD == 4) wgrad_loader_ct<UX, 4, X3>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-  else if (PD == 8) wgrad_loader_ct<UX, 8, X3>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-  else if (PD == 16) wgrad_loader_ct<UX, 16, X3>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-  else wgrad_loader_ct<UX, 32, X3>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PX);
-}
-
-__global__ void __launch_bounds__(kThreads, 1) wgrad_tc_kernel(const WgradTcParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  Ctl* ctl = reinterpret_cast<Ctl*>(smem);
-  float4* s_aff = reinterpret_cast<float4*>(smem + 128);   // [piece][scale, shift] of this ci block
-  const uint32_t base = (smem_u32(smem) + 128 + 1024 + 1023) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool stacked = p.taps_w > 1;
-
-  // work assignment: blockIdx.x -> (range r, cout block cb, channel block cc); cc fastest so the
-  // CTAs that share a pixel range (and therefore the dy tiles) run at the same time.
-  const int cc = blockIdx.x % p.n_cc;
-  const int cb = (blockIdx.x / p.n_cc) % p.co_blocks;
-  const int r = blockIdx.x / (p.n_cc * p.co_blocks);
-  const int per = (p.num_tiles + p.ranges - 1) / p.ranges;
-  // interleaved (default): CTA r takes tiles r, r + ranges, ...: at any moment the CTAs work on
-  // neighbouring tiles, so their 8-pixel-wide column segments complete DRAM pages and share halo
-  // columns in L2; contiguous ranges (ATOMAI_B200_WGRAD_ORDER=0) spread 148 CTAs over 148 far-apart
-  // image regions
-  const int ts = p.interleave ? p.ranges : 1;
-  const int t_begin = p.interleave ? r : r * per;
-  const int t_end = p.interleave ? p.num_tiles : min(p.num_tiles, t_begin + per);
-  const int co0 = cb * p.cob;
-  const int co_n = min(p.cob, p.Cout - co0);        // valid output channels in this block
-  const int ci0 = cc * p.cib;
-  const int ci_n = min(p.cib, p.Cin - ci0);         // valid input channels in this block
-  const int PD = co_n >> 2, PX = ci_n >> 2;         // 16 B pieces per pixel
-  const int Npad = (co_n + 31) & ~31;               // GEMM N (zero padded to the 32-wide atom)
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < p.n_stages; ++i) {
-      mbar_init(smem_u32(&ctl->full[i]), 4);      // the 4 warps of the group staging that slot
-      mbar_init(smem_u32(&ctl->empty[i]), 1);
-    }
-    mbar_init(smem_u32(&ctl->done), 1);
-    fence_barrier_init();
-  }
-  if (warp == kAllocWarp) tmem_alloc(smem_u32(&ctl->tmem_base), p.tmem_cols);
-  // zero both stages once: channel padding (co >= co_n, ci >= ci_n) must contribute exact zeros,
-  // and the don't-care rows behind the halo tile must at least be finite
-  for (int i = threadIdx.x; i < p.n_stages * p.stage_bytes / 16; i += kThreads)
-    sts128u(base + i * 16, 0u, 0u, 0u, 0u);
-  // BN scale / shift of this CTA's input channels, one (scale, shift) float4 pair per 16 B piece
-  for (int j = threadIdx.x; j < PX; j += kThreads) {
-    int c = ci0 + j * 4;
-    const SrcDev* sp = &p.S.s[0];
-    if (p.S.nsrc > 1 && c >= p.S.s[0].C) { sp = &p.S.s[1]; c -= p.S.s[0].C; }
-    float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (sp->scale) {
-      sc = __ldg(reinterpret_cast<const float4*>(sp->scale + c));
-      sh = __ldg(reinterpret_cast<const float4*>(sp->shift + c));
-    }
-    s_aff[2 * j] = sc;
-    s_aff[2 * j + 1] = sh;
-  }
-  fence_proxy_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
-
-  if (warp >= kFirstLoadWarp || warp < kNumEpiWarps) {
-    // ===================== loaders: dy tile + x halo tile =====================
-    // Three groups of 4 warps (warps 8-11, 12-15 and — until the final flush — the epilogue
-    // warps 0-3): group g stages the tiles with local index = g (mod 3).
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsLoad));
-    const int grp = warp >= kFirstLoadWarp ? (warp - kFirstLoadWarp) >> 2 : 2;
-    const int gt = threadIdx.x & (kGroupThreads - 1);   // warps 0-3, 8-11, 12-15 -> 0..127
-    const bool pooled = p.S.s[0].pool || (p.S.nsrc > 1 && p.S.s[1].pool);
-    const bool pow2 = PX > 0 && PD > 0 && (PX & (PX - 1)) == 0 && (PD & (PD - 1)) == 0 && PX <= 32 &&
-                      PD <= 32;
-    if (pow2 && !p.legacy_loader) {
-      // elements per thread per tile: pooled sources keep 4 loads per element in flight
-      const int ux = (p.HP * PX + kGroupThreads - 1) / kGroupThreads;
-      const bool all_pooled = p.S.s[0].pool == 1 && (p.S.nsrc == 1 || p.S.s[1].pool == 1);
-      const int qs = kGroupThreads / PX;
-      const int uxe = (p.HP + qs - 1) / qs;       // exact halo elements per thread
-      const bool ct = !pooled && !p.x3 && PD >= 4 && !p.rt_loader &&
-                      (uxe == 6 || uxe == 8 || uxe == 12);
-      if (ct && uxe == 6) wgrad_loader_ct_ud<6, false>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (ct && uxe == 8) wgrad_loader_ct_ud<8, false>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (ct && uxe == 12) wgrad_loader_ct_ud<12, false>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (!p.x3 && PD >= 4 && !p.rt_loader && !pooled && uxe == 32)
-        wgrad_loader_ctb_ud<32, 4, false>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (!p.x3 && PD >= 4 && !p.rt_loader && !pooled && uxe == 16)
-        wgrad_loader_ctb_ud<16, 8, false>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (!p.x3 && PD >= 4 && !p.rt_loader && all_pooled && uxe == 6)
-        wgrad_loader_ctb_ud<6, 3, true>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (!p.x3 && PD >= 4 && !p.rt_loader && all_pooled && uxe == 12)
-        wgrad_loader_ctb_ud<12, 3, true>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (pooled) wgrad_loader_elem<4>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (ux <= 8) wgrad_loader_elem<8>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (ux <= 12) wgrad_loader_elem<12>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else wgrad_loader_elem<16>(p, ctl, base, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-    } else if (!pooled && p.HP <= 2 * kGroupThreads && PX <= 8 && PD <= 16) {
-      if (PD <= 4) wgrad_loader_fast<4>(p, ctl, base, s_aff, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else if (PD <= 8) wgrad_loader_fast<8>(p, ctl, base, s_aff, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-      else wgrad_loader_fast<16>(p, ctl, base, s_aff, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-    } else {
-      wgrad_loader(p, ctl, base, s_aff, grp, gt, t_begin, t_end, ts, co0, ci0, PD, PX);
-    }
-    if (warp < kNumEpiWarps && t_end > t_begin) {
-      // ===================== epilogue: TMEM -> atomics into dW (OIHW) =====================
-      // accumulator row m = chunk * 32 + lane: chunk = warp = horizontal tap (stacked) or
-      // 32-channel sub-block; column = ty * Npad + (co - co0)  (fs: (taps_h-1-ty) * 32 + ...)
-      mbar_wait(smem_u32(&ctl->done), 0);
-      tc_fence_after();
-      const int taps = p.taps_h * p.taps_w;
-      const int tx = stacked ? warp : 0;
-      const int ci = stacked ? ci0 + lane : ci0 + warp * 32 + lane;
-      const bool row_ok = ci < ci0 + ci_n && tx < p.taps_w;
-      if (stacked ? warp < p.taps_w : warp * 32 < ci_n) {
-        for (int ty = 0; ty < p.taps_h; ++ty) {
-          const int col0 = p.fs ? (p.taps_h - 1 - ty) * 32 : ty * Npad;
-          for (int c0 = 0; c0 < co_n; c0 += 16) {
-            float v[16];
-            tmem_ld16(tmem_base + col0 + c0 + ((uint32_t)(warp * 32) << 16), v);
-            if (row_ok) {
-              float* o = p.dw + ((size_t)(co0 + c0) * p.Cin + ci) * taps + ty * p.taps_w + tx;
-#pragma unroll
-              for (int i = 0; i < 16; ++i)
-                if (c0 + i < co_n) atomicAdd(o + (size_t)i * p.Cin * taps, v[i]);
-            }
-          }
-        }
-      }
-    }
-  } else if (warp >= kNumEpiWarps) {
-   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsMma));
-   if (warp == kMmaWarp) {
-    if (elect_one()) {   // one elected thread issues every MMA / commit
-      const uint32_t S = p.n_stages;
-      const int th = p.taps_h;
-      const uint32_t idesc = umma_idesc_tf32(128, p.fs ? th * 32 : Npad, 1, 1);
-      const uint64_t a_tmpl = umma_desc_ex(0, stacked ? p.dil * 128 : p.x_chunk, 512, 1, 0);
-      const uint64_t b_tmpl = umma_desc_ex(0, p.fs ? p.dil * 1024 : kChunk, 512, 1, 0);
-      const uint32_t a_row16 = stacked ? (uint32_t)p.TWp * 8 : 64u;   // next tile row of x
-      const uint32_t a_ty16 = (uint32_t)(p.dil * p.TWp) * 8;          // next kernel row
-      const uint32_t a_hi = (uint32_t)(a_tmpl >> 32), b_hi = (uint32_t)(b_tmpl >> 32);
-      uint32_t st = 0, ph = 0;
-      const int n_pass = p.x3 ? 3 : 1;
-      const uint32_t xmul = p.x3 ? 2u : 1u;
-      for (int tile = t_begin; tile < t_end; tile += ts) {
-        mbar_wait(smem_u32(&ctl->full[st]), ph);
-        tc_fence_after();
-       for (int ps = 0; ps < n_pass; ++ps) {
-        // pass 0: x_hi * dy_hi, 1: x_lo * dy_hi, 2: x_hi * dy_lo
-        const uint32_t x0 = base + st * p.stage_bytes + (ps == 1 ? p.x_bytes : 0);
-        const uint32_t d0 = base + st * p.stage_bytes + xmul * p.x_bytes + (ps == 2 ? p.dy_bytes : 0);
-        const uint32_t a0 = (uint32_t)a_tmpl + (x0 >> 4);
-        const uint32_t b0 = (uint32_t)b_tmpl + (d0 >> 4);
-        uint32_t accum = (tile > t_begin || ps > 0) ? 1u : 0u;
-        if (p.fs) {
-          // one MMA per halo row r: A = x row r (tx on M), B = dy rows r-(th-1-c)*dil (ty on N)
-          uint32_t ad = a0, bd = b0;
-          const int rows = p.THp;
-#pragma unroll 2
-          for (int r = 0; r < rows; ++r) {
-            umma_tf32_lh(tmem_base, ad, a_hi, bd, b_hi, idesc, accum);
-            accum = 1u;
-            ad += a_row16;
-            bd += 64;
-          }
-        } else {
-          uint32_t a_ty = a0;
-          uint32_t dcol = tmem_base;
-          for (int ty = 0; ty < th; ++ty, a_ty += a_ty16, dcol += Npad) {
-            uint32_t ad = a_ty, bd = b0;
-            uint32_t acc2 = accum;
-#pragma unroll
-            for (int h = 0; h < kTileH; ++h) {
-              umma_tf32_lh(dcol, ad, a_hi, bd, b_hi, idesc, acc2);
-              acc2 = 1u;
-              ad += a_row16;         // next halo row (8 output pixels further down)
-              bd += 64;              // next 8 pixels of the dy tile (8 x 128 B)
-            }
-          }
-        }
-       }
-        umma_commit(smem_u32(&ctl->empty[st]));
-        if (++st == S) { st = 0; ph ^= 1; }
-      }
-      umma_commit(smem_u32(&ctl->done));
-    }
-    __syncwarp();
-   }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kAllocWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
+      for (int e = 0; e < 2; ++e)
+        slot[(16 * warp + (lane >> 2) + 8 * h) * CIB + 8 * j + 2 * (lane & 3) + e] = acc[4 * j + 2 * h + e];
+  __shared__ unsigned s_last;
+  ordered_finish(p.red, blockIdx.y, gridDim.x, n, tid, kThreads, gridDim.x, [] { __syncthreads(); },
+                 [&](int i, double v) {
+                   const int co = co0 + i / CIB, ci = ci0 + i % CIB;
+                   if (co < p.Cout && ci < p.Cin) p.dw[((size_t)co * p.Cin + ci) * taps + t] += (float)v;
+                 },
+                 &s_last);
 }
 
 int wgrad_plan(const ab_conv_t* d, WgradTcParams* p, int* smem_bytes) {
@@ -1127,74 +181,42 @@ int wgrad_plan(const ab_conv_t* d, WgradTcParams* p, int* smem_bytes) {
   p->N = d->N; p->H = d->H; p->W = d->W; p->Cout = d->Cout; p->Cin = p->S.Ctot;
   p->taps_h = d->ks_h; p->taps_w = d->ks_w; p->dil = d->dil;
   p->x3 = d->math == AB_MATH_TF32X3 ? 1 : 0;
-  {
-    const char* e = getenv("ATOMAI_B200_WGRAD_LOADER");
-    p->legacy_loader = (e && e[0] == '0') ? 1 : 0;
-    p->rt_loader = (e && e[0] == '1') ? 1 : 0;
-    const char* o = getenv("ATOMAI_B200_WGRAD_ORDER");
-    p->interleave = (o && o[0] == '0') ? 0 : 1;
-    const char* f = getenv("ATOMAI_B200_WGRAD_PF");
-    p->l2_prefetch = (f && f[0] == '1') ? 1 : 0;
-  }
   AB_CHECK(d->ks_w <= 4 && d->ks_h <= 4, "wgrad_tc: kernel %dx%d too large", d->ks_h, d->ks_w);
-  p->tiles_h = (d->H + kTileH - 1) / kTileH;
-  p->tiles_w = (d->W + kTileW - 1) / kTileW;
-  p->num_tiles = d->N * p->tiles_h * p->tiles_w;
-  AB_CHECK((uint64_t)p->num_tiles * (uint64_t)(p->tiles_h * p->tiles_w) < (1ull << 32) &&
-               (uint64_t)p->num_tiles * 9 < (1ull << 32),
-           "wgrad_tc: too many tiles");
-  p->THp = kTileH + d->dil * (d->ks_h - 1);
-  p->TWp = kTileW + d->dil * (d->ks_w - 1);
-  p->HP = p->THp * p->TWp;
-  const bool stacked = d->ks_w > 1;
-  // A stage is [x tile][dy tile] (x3: [x_hi][x_lo][dy_hi][dy_lo]): the don't-care rows of the
-  // M = 128 operand (chunk 3 of a 3-wide kernel, chunks >= cib/32 of a 1x1 kernel) then alias
-  // whatever follows the x tile — finite and in bounds.  Search the widest (output-channel block,
-  // input-channel block) for which two stages fit.
-  p->fs = stacked && d->Cout <= 32 && d->ks_h > 1;
-  p->dpad = p->fs ? (d->ks_h - 1) * d->dil : 0;
-  const int mult = p->x3 ? 2 : 1;
-  const int smem_cap = 225 * 1024 - 128 - 2048;
-  bool ok = false;
-  int npad = 0;
-  for (int cob = 128; cob >= 64 && !ok; cob >>= 1) {
-    const int co_max = d->Cout < cob ? d->Cout : cob;
-    npad = (co_max + 31) & ~31;
-    int dy_bytes = (npad / 32) * kChunk;
-    if (p->fs) dy_bytes = (kTileH + 2 * p->dpad + (d->ks_h - 1) * d->dil) * 1024;   // + chunk over-read
-    for (int cib = stacked ? 32 : 128; cib >= 32 && !ok; cib >>= 1) {
-      int x_chunk = 0, x_bytes;
-      if (stacked) {
-        x_bytes = (p->HP * 128 + 1023) & ~1023;
-        if (3 * d->dil * 128 + 1024 > dy_bytes) continue;
-      } else {
-        x_chunk = (p->HP * 128 + 1023) & ~1023;
-        x_bytes = (cib / 32) * x_chunk;
-      }
-      const int stage = mult * (x_bytes + dy_bytes);
-      if (2 * stage > smem_cap) continue;
-      if (!stacked && (p->x3 ? x_bytes : 0) + 4 * x_chunk > stage) continue;   // aliased chunks in bounds
-      p->cob = cob; p->cib = cib; p->x_chunk = x_chunk; p->x_bytes = x_bytes;
-      p->dy_bytes = dy_bytes; p->stage_bytes = stage;
-      ok = true;
-    }
-  }
-  AB_CHECK(ok, "wgrad_tc: no shared-memory plan (Cin=%d Cout=%d dil=%d)", p->Cin, d->Cout, d->dil);
-  p->co_blocks = (d->Cout + p->cob - 1) / p->cob;
-  int ns = smem_cap / p->stage_bytes;
-  if (ns > kMaxStages) ns = kMaxStages;
-  p->n_stages = ns;
-  *smem_bytes = ns * p->stage_bytes + 128 + 2048;
-  p->n_cc = (p->Cin + p->cib - 1) / p->cib;
-  int cols = 32;
-  while (cols < (p->fs ? d->ks_h * 32 : d->ks_h * npad)) cols <<= 1;
-  AB_CHECK(cols <= 512, "wgrad_tc: too many accumulator columns");
-  p->tmem_cols = cols;
-  const int groups = p->n_cc * p->co_blocks;
-  int ranges = ab_num_sms() / groups;
+  p->tiles_h = (d->H + kTile - 1) / kTile;
+  p->tiles_w = (d->W + kTile - 1) / kTile;
+  const int64_t nt = (int64_t)d->N * p->tiles_h * p->tiles_w;
+  AB_CHECK(nt < (1ll << 31) / 4096, "wgrad_tc: too many tiles");
+  p->num_tiles = (int)nt;
+  p->cib = p->Cin <= 16 ? 16 : (p->Cin <= 32 ? 32 : 64);
+  p->n_cib = (p->Cin + p->cib - 1) / p->cib;
+  p->n_cob = (d->Cout + kM - 1) / kM;
+  p->a_bytes = (kM / 8) * kSbo;
+  p->b_bytes = (p->cib / 8) * kSbo;
+  p->stage_bytes = ((p->a_bytes + p->b_bytes) * (p->x3 ? 2 : 1) + 127) & ~127;
+  *smem_bytes = 2 * p->stage_bytes;
+  // about six CTAs per SM in total (two waves of the three that fit at N = 64): a CTA is one
+  // warpgroup that waits on its own global loads, so latency is hidden by resident CTAs; every
+  // CTA keeps at least a few tiles
+  const int groups = d->ks_h * d->ks_w * p->n_cob * p->n_cib;
+  int ranges = (6 * ab_num_sms() + groups - 1) / groups;
+  if (ranges > p->num_tiles / 4) ranges = p->num_tiles / 4;
   if (ranges < 1) ranges = 1;
-  if (ranges > p->num_tiles) ranges = p->num_tiles > 0 ? p->num_tiles : 1;
   p->ranges = ranges;
+  return 0;
+}
+
+template <int CIB>
+int launch(const WgradTcParams& p, int smem, cudaStream_t stream) {
+  // opted in once per device for the largest plan of this N (tf32x3 stages), not for the first
+  const int max_smem = 2 * ((((kM + CIB) / 8) * kSbo * 2 + 127) & ~127);
+  AB_CHECK(smem <= max_smem, "wgrad_tc: %d B of shared memory exceeds the plan bound", smem);
+  static unsigned char optin[64];
+  if (ab_optin_smem(reinterpret_cast<const void*>(wgrad_tc_kernel<CIB>), max_smem, optin)) return 1;
+  const dim3 grid(p.ranges, p.taps_h * p.taps_w * p.n_cob * p.n_cib);
+  WgradTcParams q = p;
+  if (ab_ordered_ws(stream, (int64_t)grid.x * grid.y * kM * CIB, grid.y, &q.red)) return 1;
+  wgrad_tc_kernel<CIB><<<grid, kThreads, smem, stream>>>(q);
+  AB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -1221,10 +243,7 @@ int ab_conv_tc_wgrad(const ab_conv_t* d, const float* dy, int ld_dy, float* dw,
   AB_CHECK(((uintptr_t)dy & 15) == 0 && ld_dy % 4 == 0, "wgrad_tc: unaligned dy");
   p.dy = dy; p.ld_dy = ld_dy; p.dw = dw;
   if (p.num_tiles == 0) return 0;
-  static unsigned char optin[64];
-  if (ab_optin_smem(reinterpret_cast<const void*>(wgrad_tc_kernel), 226 * 1024, optin)) return 1;
-  const int grid = p.ranges * p.n_cc * p.co_blocks;
-  wgrad_tc_kernel<<<grid, kThreads, smem, stream>>>(p);
-  AB_LAUNCH_CHECK();
-  return 0;
+  if (p.cib == 16) return launch<16>(p, smem, stream);
+  if (p.cib == 32) return launch<32>(p, smem, stream);
+  return launch<64>(p, smem, stream);
 }

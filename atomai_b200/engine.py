@@ -1,5 +1,5 @@
 """
-Define-by-run native graph ("tape") that executes a network as a sequence of sm_100a kernels and
+Define-by-run native graph ("tape") that executes a network as a sequence of sm_90a kernels and
 replays it backwards.  It is the host-side orchestration of the C ABI, not a compute path of its
 own: torch supplies device memory, the current stream and the autograd *boundary* (one
 torch.autograd.Function per network call); all arithmetic on activations happens in
@@ -35,11 +35,10 @@ _NO_POOLSTATS = os.environ.get("ATOMAI_B200_NO_POOLSTATS", "0") == "1"    # A/B 
 def set_fusion(upsample: Optional[bool] = None) -> None:
     """upsample=True: `F.interpolate(scale_factor=2)` of an UpsampleBlock is NOT written out; the
     convolution that consumes it (and its weight-gradient kernel) interpolates the (H/2, W/2)
-    tensor while staging its input tile (descriptor code `pool = 2 / 3`).  Measured on the bench
-    workload (32 x 512^2, round 2): the fit cycle takes 25.6 ms fused against 23.7 ms with the
-    upsampled tensor materialised — four dependent loads + the interpolation per staged element in
-    the register-staged loaders cost more than the 0.8 ms `upsample_fwd` pass they replace, and
-    the layer loses its TMA-staged path — so the default is False."""
+    tensor while staging its input tile (descriptor code `pool = 2 / 3`).  Four dependent loads +
+    the interpolation per staged element in the register-staged loaders can cost more than the
+    `upsample_fwd` pass they replace, and the layer loses its TMA-staged path, so the default is
+    False."""
     if upsample is not None:
         _MATH["fuse_up"] = bool(upsample)
 
@@ -47,7 +46,7 @@ def set_fusion(upsample: Optional[bool] = None) -> None:
 def set_math(mode: str = "tf32x3", wgrad_tc: Optional[bool] = None,
              wgrad_math: Optional[str] = "auto") -> None:
     """Arithmetic of the convolution family:
-      'tf32'   tcgen05 tensor cores, operands RN-rounded to TF32 (what stock PyTorch/cuDNN does by
+      'tf32'   wgmma tensor cores, operands RN-rounded to TF32 (what stock PyTorch/cuDNN does by
                default on CUDA); ~1e-3 relative on the logits of a 17-layer Unet;
       'tf32x3' the same kernels with every operand split into a TF32 high and low part (three MMAs
                per product, fp32 accumulate): matches the reference's fp32 CPU results to ~1e-6;
@@ -574,7 +573,7 @@ class Tape:
 
     def mlp(self, x: Act, lins: Sequence, acts: Sequence) -> Act:
         """Chain of nn.Linear (+ReLU / tanh) layers on a (B,1,1,K) activation — the DKL feature
-        extractor (atomai/nets/gp.py:14-26: feat -> 1000 -> 500 -> 50 -> embedim) — on the tcgen05
+        extractor (atomai/nets/gp.py:14-26: feat -> 1000 -> 500 -> 50 -> embedim) — on the wgmma
         convolution kernel: the B rows become the pixels of a (1, B/8, 8, K) image, each layer is a
         1x1 convolution with fused bias + activation, wide layers run as column blocks of <= 256
         outputs writing channel slices of one buffer.  Channel counts are zero-padded to the MMA
@@ -1020,7 +1019,7 @@ def run_multi(module, emit, inputs, comm=None):
     params = [p for p in module.parameters()]
     for t in inputs:
         if not t.is_cuda:
-            raise RuntimeError("atomai_b200 networks run on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("atomai_b200 networks run on CUDA (sm_90a) only; there is no CPU path")
     return _MultiFn.apply(module, emit, comm, torch.is_grad_enabled(), len(inputs), *inputs, *params)
 
 
@@ -1030,7 +1029,7 @@ def _to_nhwc(x: torch.Tensor) -> torch.Tensor:
         x = x.unsqueeze(2)
     assert x.dim() == 4, f"expected NCHW input, got shape {tuple(x.shape)}"
     if not x.is_cuda:
-        raise RuntimeError("atomai_b200 networks run on CUDA (sm_100a) only; there is no CPU path")
+        raise RuntimeError("atomai_b200 networks run on CUDA (sm_90a) only; there is no CPU path")
     if x.dtype != torch.float32:
         x = x.float()
     xp = x.permute(0, 2, 3, 1)

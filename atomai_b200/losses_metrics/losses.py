@@ -2,7 +2,7 @@
 Loss functions for the native path.  `select_loss` has the reference's contract
 (atomai/losses_metrics/losses.py:139-174): the returned criteria are nn.Modules whose names and
 reprs match torch's (`str(criterion) == "CrossEntropyLoss()"`, test/trainers/test_trainer.py:59-74)
-but whose forward/backward run as fused sm_100a kernels: one pass computes the summed loss, the
+but whose forward/backward run as fused sm_90a kernels: one pass computes the summed loss, the
 backward pass recomputes the softmax and writes d(logits) scaled by the upstream gradient read from
 device memory (no host synchronisation).
 """
@@ -25,7 +25,7 @@ class _CEFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, target):
         if not logits.is_cuda:
-            raise RuntimeError("atomai_b200 losses run on CUDA (sm_100a) only")
+            raise RuntimeError("atomai_b200 losses run on CUDA (sm_90a) only")
         l = _nhwc_view(logits.detach().float())
         tgt = target.detach()
         if tgt.dtype != torch.int64:
@@ -56,7 +56,7 @@ class _PointwiseFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, target, kind):
         if not pred.is_cuda:
-            raise RuntimeError("atomai_b200 losses run on CUDA (sm_100a) only")
+            raise RuntimeError("atomai_b200 losses run on CUDA (sm_90a) only")
         # elementwise: memory order is irrelevant as long as both operands share it
         if pred.stride() == target.stride() and pred.is_non_overlapping_and_dense() \
                 and target.is_non_overlapping_and_dense():

@@ -19,7 +19,7 @@ class _RowLossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, x_hat, kind):
         if not x_hat.is_cuda:
-            raise RuntimeError("atomai_b200 losses run on CUDA (sm_100a) only")
+            raise RuntimeError("atomai_b200 losses run on CUDA (sm_90a) only")
         xc = x.detach().float().contiguous()
         xh = x_hat.detach().float().contiguous()
         assert xc.numel() == xh.numel(), "input and reconstruction differ in size"

@@ -1,6 +1,6 @@
 """
 rVAE — rotationally (and translationally) invariant VAE (atomai/models/dgm/rvae.py:22-219) on the
-native sm_100a path: convolutional (or MLP) encoder, fused coordinate-transform + per-pixel MLP
+native sm_90a path: convolutional (or MLP) encoder, fused coordinate-transform + per-pixel MLP
 spatial decoder, fused reconstruction reduction.  The (B, H*W, 2) coordinate tensor of the
 reference (rvae.py:118,140) is never materialised.
 """

@@ -1,6 +1,6 @@
 """
 BaseVAE / VAE — user-facing variational autoencoder (atomai/models/dgm/vae.py:28-747) on the
-native sm_100a path.  Kept: construction kwargs, encode / decode / reconstruct, fit, save_model,
+native sm_90a path.  Kept: construction kwargs, encode / decode / reconstruct, fit, save_model,
 loss history.  The plotting helpers (manifold2d, visualize_manifold_learning, ...) depend on
 matplotlib and are outside the hot-path scope (SURVEY.md §2.1).
 """

@@ -1,6 +1,6 @@
 """
 ImSpec — image -> spectrum / spectrum -> image model, drop-in for atomai.models.ImSpec
-(atomai/models/imspec.py:18-170), trained through the native sm_100a SignalED graph.
+(atomai/models/imspec.py:18-170), trained through the native sm_90a SignalED graph.
 """
 from typing import Optional, Tuple, Type, Union
 

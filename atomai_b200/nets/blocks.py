@@ -1,6 +1,6 @@
 """
 Customized NN blocks, same constructor signatures, module tree and state_dict keys as the
-reference (atomai/nets/blocks.py:17-132, 257-329), executed by hand-written sm_100a kernels.
+reference (atomai/nets/blocks.py:17-132, 257-329), executed by hand-written sm_90a kernels.
 
 The torch sub-modules (nn.Conv2d, nn.LeakyReLU, nn.BatchNorm2d inside `self.block` /
 `self.atrous_module`, `self.conv`) are parameter containers only: `forward` never calls them.
@@ -122,7 +122,7 @@ class ResBlock(nn.Module):
     """
     Builds a residual block: 1x1 conv -> [3x3 conv -> BN -> LeakyReLU -> 3x3 conv -> BN] + skip ->
     LeakyReLU (atomai/nets/blocks.py:135-214; identical signature and parameter names).  Natively:
-    three tcgen05 convolutions with the BatchNorm statistics in their epilogues, and the
+    three wgmma convolutions with the BatchNorm statistics in their epilogues, and the
     BN-affine + residual add + LeakyReLU tails as one HBM pass each (csrc/resnet.cu).
     """
     def __init__(self,

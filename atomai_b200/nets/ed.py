@@ -1,9 +1,9 @@
 """
 Encoder / decoder networks for ImSpec and the (r)VAEs — constructor signatures, module names and
 state_dict layout of the reference (atomai/nets/ed.py:20-228, 231-343, 471-687, 690-790), executed
-by the native sm_100a tape (atomai_b200/engine.py).
+by the native sm_90a tape (atomai_b200/engine.py).
 
-Each network is one autograd node per call; inside it the ConvBlocks run on the tcgen05
+Each network is one autograd node per call; inside it the ConvBlocks run on the wgmma
 convolution kernels, `x.reshape(-1, C*H*W) -> nn.Linear` becomes an NHWC->NCHW transpose kernel +
 a split-K GEMM, and the rVAE spatial decoder (coord_latent + transform_coordinates + per-pixel MLP)
 is a fused coordinate kernel followed by 1x1 tensor-core convolutions with tanh epilogues.

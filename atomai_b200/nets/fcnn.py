@@ -1,7 +1,7 @@
 """
 Fully convolutional neural networks — Unet and dilnet with the reference's constructor
 signatures, module names and checkpoint layout (atomai/nets/fcnn.py:18-226, 379-442), executed
-as one native sm_100a graph per call (see atomai_b200/engine.py).
+as one native sm_90a graph per call (see atomai_b200/engine.py).
 
 ResHedNet / SegResNet (ResBlock based, atomai/nets/fcnn.py:229-376) run on the same native tape.
 """

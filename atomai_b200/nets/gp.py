@@ -158,8 +158,8 @@ class GPRegressionModel(torch.nn.Module):
     output, Gaussian likelihood.  The reference wraps the base kernel in gpytorch's KISS-GP
     (GridInterpolationKernel) and leaves every GP computation (CG, Lanczos, posterior caches) to
     gpytorch, which is neither vendored nor installed here.  This class evaluates the SAME base
-    kernel densely on the native kernels (fcFeatureExtractor as tcgen05 1x1 convolutions, Gram with
-    the exponentiation fused in the TMEM epilogue) and does exact-GP algebra (Cholesky) with
+    kernel densely on the native kernels (fcFeatureExtractor as wgmma 1x1 convolutions, Gram with
+    the exponentiation fused in the register epilogue) and does exact-GP algebra (Cholesky) with
     torch.linalg: an exact GP instead of the SKI approximation of it, for N up to ~10^4 points.
     Hyper-parameter parametrisation follows gpytorch's defaults: softplus raw parameters,
     noise >= 1e-4, zero raw initial values; `grid_size` is accepted and ignored.

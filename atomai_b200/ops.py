@@ -2,7 +2,7 @@
 Thin tensor-level wrappers over the C ABI (include/atomai_b200.h).
 
 torch is used here for device memory and the current stream only; every
-function launches hand-written sm_100a kernels from libatomai_b200.so and
+function launches hand-written sm_90a kernels from libatomai_b200.so and
 raises if that library is unavailable.  Activations are NHWC fp32 tensors of
 shape (N, H, W, C); a channel slice of a wider tensor is passed as a view whose
 last-dim stride is 1 (its pixel stride `ld` is read from the strides).
@@ -80,14 +80,14 @@ def conv_desc(srcs: Sequence[Source], N, H, W, Cout, ks=(3, 3), dil=1, lrelu=1.0
 
 
 def tc_supported(srcs: Sequence[Source], Cout: int) -> bool:
-    """Shapes the tcgen05 conv path takes (mirrors ab_conv_tc_supported)."""
+    """Shapes the wgmma conv path takes (mirrors ab_conv_tc_supported)."""
     ctot = sum(s.C for s in srcs)
     return (all(s.C % 4 == 0 and _ld(s.t) % 4 == 0 and s.t.data_ptr() % 16 == 0 for s in srcs)
             and ctot % 8 == 0 and Cout % 16 == 0 and 16 <= Cout <= 256)
 
 
 def conv_supported(d: _C.Conv, which: int = 0) -> bool:
-    """Does the tcgen05 kernel take this descriptor?  which: 0 forward/dgrad, 1 weight gradient
+    """Does the wgmma kernel take this descriptor?  which: 0 forward/dgrad, 1 weight gradient
     (atomai_b200_conv_supported — the single source of truth, no Python mirror)."""
     return bool(lib().atomai_b200_conv_supported(C.byref(d), which))
 
@@ -370,11 +370,3 @@ def selftest_tma(x, c0, w0, h0, n0, TWp, THp, swizzle_mode, smem_offset, out) ->
     N, H, W, Cc = x.shape
     check(lib().atomai_b200_selftest_tma(ptr(x), N, H, W, Cc, c0, w0, h0, n0, TWp, THp, swizzle_mode,
                                          smem_offset, ptr(out), stream_ptr()))
-
-
-def selftest_sw128(A, B, D, N, K, variant) -> None:
-    check(lib().atomai_b200_selftest_sw128(ptr(A), ptr(B), ptr(D), N, K, variant, stream_ptr()))
-
-
-def selftest_umma(A, B, D, N, K, variant) -> None:
-    check(lib().atomai_b200_selftest_umma(ptr(A), ptr(B), ptr(D), N, K, variant, stream_ptr()))

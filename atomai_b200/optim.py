@@ -1,5 +1,5 @@
 """
-Fused multi-tensor Adam: one sm_100a kernel launch updates every parameter tensor of the model
+Fused multi-tensor Adam: one sm_90a kernel launch updates every parameter tensor of the model
 (the reference's torch.optim.Adam, atomai/trainers/trainer.py:539, is ~60 small launches for the
 default Unet).  Same update rule, hyper-parameters and state names (`exp_avg`, `exp_avg_sq`,
 `step`) as torch.optim.Adam without amsgrad.
@@ -47,7 +47,7 @@ class FusedAdam(torch.optim.Optimizer):
                 continue
             for p in ps:
                 if not p.is_cuda:
-                    raise RuntimeError("FusedAdam runs on CUDA (sm_100a) only")
+                    raise RuntimeError("FusedAdam runs on CUDA (sm_90a) only")
                 st = self.state[p]
                 if len(st) == 0:
                     st["step"] = 0

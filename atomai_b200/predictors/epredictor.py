@@ -1,7 +1,7 @@
 """
 Prediction with an ensemble of models (atomai/predictors/epredictor.py:21-267): EnsemblePredictor
 (mean and variance over the members' outputs) and ensemble_locate.  Every member's forward runs on
-the native sm_100a graph; the running mean / M2 accumulation over members stays on the device, so
+the native sm_90a graph; the running mean / M2 accumulation over members stays on the device, so
 only the final mean and variance cross PCIe (the reference copies every member's full output).
 """
 from typing import Dict, Tuple, Type, Union
@@ -37,7 +37,7 @@ class EnsemblePredictor(BasePredictor):
         if inout in (["image", "spectra"], ["spectra", "image"]) and not all([in_dim, out_dim]):
             raise TypeError("Specify input (in_dim) & output (out_dim) dimensions")
         if not torch.cuda.is_available():
-            raise RuntimeError("atomai_b200 predicts on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("atomai_b200 predicts on CUDA (sm_90a) only; there is no CPU path")
         self.device = kwargs.get("device") or "cuda"
         self.model = skeleton
         self.ensemble = ensemble

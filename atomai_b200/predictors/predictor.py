@@ -1,7 +1,7 @@
 """
 Inference wrappers and NN-output -> atom coordinates, with the reference's interface
 (atomai/predictors/predictor.py:23-298, 531-639).  The network forward runs on the GPU (native
-sm_100a graph) and so does the Locator's front end: one kernel turns the NHWC logits into class
+sm_90a graph) and so does the Locator's front end: one kernel turns the NHWC logits into class
 probabilities AND the thresholded binary masks (atomai_b200_prob_mask), batches are copied to
 pinned host buffers asynchronously and synchronised once.  Connected components -> centre of mass
 -> edge filter stay the reference's CPU algorithm (scipy.ndimage) on those masks, bit-exact with
@@ -147,7 +147,7 @@ class SegPredictor(BasePredictor):
         batch's probabilities and masks are copied into pinned host buffers on the compute stream
         and the host waits once at the end.  The masks are kept in `self.masks_`."""
         if self.device == "cpu" or not torch.cuda.is_available():
-            raise RuntimeError("atomai_b200 predicts on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("atomai_b200 predicts on CUDA (sm_90a) only; there is no CPU path")
         batch_size = len(data) // num_batches
         if batch_size < 1:
             num_batches = batch_size = 1

@@ -2,7 +2,7 @@
 Deep-ensemble training with the reference's interface (atomai/trainers/etrainer.py:29-512):
 BaseEnsembleTrainer / EnsembleTrainer with train_baseline, train_ensemble_from_scratch,
 train_ensemble_from_baseline, train_swag, save_ensemble_metadict.  Every member is an ordinary
-BaseTrainer run on the native sm_100a path.
+BaseTrainer run on the native sm_90a path.
 
 Multi-GPU (new; the reference is single-device): ensembles are the "replicas" workload of
 SURVEY.md §8e/§8f — members are independent, so under torchrun member i is trained by rank

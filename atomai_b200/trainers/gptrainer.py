@@ -2,7 +2,7 @@
 Trainers for deep-kernel-learning GP regression with the reference's public surface
 (atomai/trainers/gptrainer.py:18-57, 126-349): GPTrainer data handling + train_step, dklGPTrainer
 compile_trainer / compile_multi_model_trainer / run / save_weights.  The feature extractor and the
-kernel Gram run on the native sm_100a kernels; the GP algebra is the dense exact GP of
+kernel Gram run on the native sm_90a kernels; the GP algebra is the dense exact GP of
 atomai_b200.nets.gp.GPRegressionModel (gpytorch, which the reference delegates it to, is not
 available in this image).
 """
@@ -106,7 +106,7 @@ class dklGPTrainer(GPTrainer):
 
     def _require_cuda(self):
         if not str(self.device).startswith("cuda"):
-            raise RuntimeError("atomai_b200 runs on CUDA (B200, sm_100a) only: the native deep-"
+            raise RuntimeError("atomai_b200 runs on CUDA (H100, sm_90a) only: the native deep-"
                                "kernel path has no CPU fallback")
 
     def _optimizer(self, param_groups, lr):

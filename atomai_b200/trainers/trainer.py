@@ -6,7 +6,7 @@ mini-batch" unless full_epoch), loss histories and checkpoint dictionary.
 
 What is different underneath:
   * `self.net(feat)`, `self.criterion(...)`, `loss.backward()` and `optimizer.step()` — the seam
-    into the hot path, trainer.py:204-207 — run as hand-written sm_100a kernels (native tape,
+    into the hot path, trainer.py:204-207 — run as hand-written sm_90a kernels (native tape,
     fused loss, fused multi-tensor Adam);
   * data parallelism over the GPUs of one box when launched under torchrun: mini-batches are
     sharded along N, gradients all-reduced once per step over NCCL (atomai_b200/parallel.py).
@@ -147,7 +147,7 @@ class BaseTrainer:
     def _require_cuda(self) -> None:
         if self.device != 'cuda':
             raise RuntimeError(
-                "atomai_b200 trains on CUDA (B200, sm_100a) only: the native kernels have no CPU "
+                "atomai_b200 trains on CUDA (H100, sm_90a) only: the native kernels have no CPU "
                 "fallback. Use the reference AtomAI for CPU training.")
 
     def train_step(self, feat: torch.Tensor, tar: torch.Tensor) -> Tuple[float]:
@@ -535,7 +535,7 @@ class SegTrainer(BaseTrainer):
         self.net, self.meta_state_dict = init_fcnn_model(model, self.nb_classes, **kwargs)
         self.net.to(self.device)
         if self.device == 'cpu':
-            warnings.warn("No GPU found. atomai_b200 cannot train without a B200 (sm_100a)",
+            warnings.warn("No GPU found. atomai_b200 cannot train without an H100 (sm_90a)",
                           UserWarning)
         self.meta_state_dict["weights"] = self.net.state_dict()
 

@@ -2,7 +2,7 @@
 viBaseTrainer — training loop of the variational autoencoders with the reference's interface
 (atomai/trainers/vitrainer.py:19-396): set_model / set_data / compile_trainer / reparameterize /
 train_epoch / evaluate_model / save_model.  Encoder, decoder, reconstruction loss and the Adam step
-run as native sm_100a kernels; under torchrun the DataLoader batches are sharded over the ranks and
+run as native sm_90a kernels; under torchrun the DataLoader batches are sharded over the ranks and
 the gradients all-reduced once per step (the encoder's fc weights dominate: ~21 MB per step).
 """
 from typing import Callable, Optional, Tuple, Type, Union
@@ -154,7 +154,7 @@ class viBaseTrainer:
     def train_epoch(self):
         """Trains a single epoch; returns the running mean of the ELBO (vitrainer.py:292-318)."""
         if self.device != "cuda":
-            raise RuntimeError("atomai_b200 trains on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("atomai_b200 trains on CUDA (sm_90a) only; there is no CPU path")
         step = self.forward_compute_elbo
         self.decoder_net.train()
         self.encoder_net.train()

@@ -10,7 +10,7 @@ Appendix A), none of which is on the Segmentor / VAE / ImSpec code path: they ar
 inert stub modules so that `import atomai` runs the reference's own code unchanged.
 
 Used by bench.py's `--impl reference` (CPU) and `--impl torch-cuda` (stock PyTorch/cuDNN on the
-B200) arms and by oracle/ref_shim.py (golden generation).  Nothing under atomai_b200/ imports it.
+GPU) arms and by oracle/ref_shim.py (golden generation).  Nothing under atomai_b200/ imports it.
 """
 import os
 import sys

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """
-bench.py — Segmentor.fit throughput on B200 (BASELINE.json metric:
+bench.py — Segmentor.fit throughput on H100 (BASELINE.json metric:
 "Segmentor.fit images/sec (512x512, 3-class)"; default workload = configs[1]: Unet nb_classes=3,
 batch 32 of 512x512 fp32 synthetic stacks per GPU).
 
@@ -8,10 +8,12 @@ batch 32 of 512x512 fp32 synthetic stacks per GPU).
   python bench.py --impl reference ...                      the UNMODIFIED reference (baseline/_ref) on
                                                             the host cores, same config (batch 32)
   python bench.py --impl torch-cuda ...                     the UNMODIFIED reference with device='cuda':
-                                                            stock PyTorch/cuDNN sm_100 kernels, the
-                                                            "existing Blackwell path" (SURVEY.md §2.2)
+                                                            stock PyTorch/cuDNN kernels, the existing
+                                                            GPU path (SURVEY.md §2.2)
   python bench.py --workload {seg512,seg256,rvae,imspec,gram}   the other BASELINE.json configs
   python bench.py --scaling strong                          global batch fixed at 32 (32/N per GPU)
+  python bench.py --dump-outputs DIR                        also write what the last timed step computed
+                                                            (losses, parameters) as DIR/<name>.npy
 
 A "step" is one Segmentor.fit training cycle of the reference (atomai/trainers/trainer.py:233-251):
 one train mini-batch (forward + backward + Adam) followed by one test mini-batch forward.
@@ -73,11 +75,12 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d["bf16_tflops_sustained"],
                     src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     def __init__(self, index):
         super().__init__(daemon=True)
         self.index, self.rows, self.stop_flag = index, [], False
@@ -194,8 +197,8 @@ def run_reference(args):
 
 
 def run_torch_cuda(args):
-    """`--impl torch-cuda`: the unmodified reference with device='cuda' on ONE B200 — every conv is a
-    stock ATen -> cuDNN call (SURVEY.md §2.2: the existing Blackwell kernels to beat).  Variants:
+    """`--impl torch-cuda`: the unmodified reference with device='cuda' on ONE GPU — every conv is a
+    stock ATen -> cuDNN call (SURVEY.md §2.2: the existing GPU kernels to beat).  Variants:
     stock (cuDNN TF32 allowed = PyTorch default; deterministic algorithms as the reference's
     set_train_rng sets them), fp32 (cudnn.allow_tf32 = False), tuned (cudnn.benchmark, non-
     deterministic), channels_last (tuned + NHWC weights)."""
@@ -255,7 +258,7 @@ def run_torch_cuda(args):
         "config": {"workload": f"unmodified reference Segmentor('Unet', nb_classes=3).fit cycle on "
                                f"device='cuda'; batch {batch} x {hw}x{hw}x1 fp32",
                    "torch": torch.__version__, "cudnn": torch.backends.cudnn.version()},
-        "gpu_baseline": {"kind": "reference on stock PyTorch/cuDNN, 1 x B200", "unit": "images/s",
+        "gpu_baseline": {"kind": "reference on stock PyTorch/cuDNN, 1 GPU", "unit": "images/s",
                          "variants": out},
         "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 8,
                 "note": "memory_alloc=0: the reference keeps the batches on the host and copies "
@@ -272,7 +275,19 @@ def _maxreduce_ms(ms, dev, world):
     return float(t.item())
 
 
-def measure_seg_mode(math, args, world, rank, dev, data, gb, per_gpu, hw):
+def dump_outputs(m, out_dir):
+    """What the last timed fit cycle handed back to its caller: the train / test losses it recorded
+    and the trained state (every parameter and BatchNorm buffer), one float32 .npy per array."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"train_loss": [float(m.loss_acc["train_loss"][-1])],
+              "test_loss": [float(m.loss_acc["test_loss"][-1])]}
+    for k, v in m.net.state_dict().items():
+        arrays["state." + k] = v.detach().float().cpu().numpy()
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.asarray(v, dtype=np.float32))
+
+
+def measure_seg_mode(math, args, world, rank, dev, data, gb, per_gpu, hw, dump_dir=None):
     """One math mode: device-resident cycle (value), train-step-only, in-situ per-kernel profile of
     one cycle (roofline) and the end-to-end cycle from pinned host buffers."""
     import atomai_b200 as ab
@@ -309,6 +324,8 @@ def measure_seg_mode(math, args, world, rank, dev, data, gb, per_gpu, hw):
     launches = _C.launch_count() - calls0
     ms_total = _maxreduce_ms(ev0.elapsed_time(ev1), dev, world)
     final_losses = [float(v) for v in m.loss_acc["train_loss"][-2:]]
+    if dump_dir and rank == 0:
+        dump_outputs(m, dump_dir)
 
     # train-step-only timing (secondary figure)
     barrier()
@@ -396,14 +413,8 @@ def roofline_from_profile(res, pk, world, per_gpu, hw):
     dom = max((k for k in kern if k.endswith("_tc_kernel")), key=lambda k: kern[k]["ms"], default=None)
     if dom is None:
         return {"bound": "tensor", "achieved": None, "peak": round(tf32_peak, 1), "unit": "TFLOP/s",
-                "frac": None, "traffic": None, "kernels": kern}
+                "frac": None, "kernels": kern}
     step_tflops = FLOP_PER_PIXEL_TRAIN * hw * hw * per_gpu * world / (res["train_step_only_ms"] / 1e3) / 1e12
-    traffic, traffic_src = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r02_roofline.json")))
-        traffic, traffic_src = tj.get("traffic_bytes_per_launch"), tj.get("source")
-    except Exception:  # noqa
-        pass
     return {"bound": "tensor", "kernel": f"{dom}, all {kern[dom]['launches']} launches of one fit cycle "
             f"(forward train + forward test + dgrad), math {res['math']}",
             "achieved": kern[dom]["algorithmic_tflops"], "peak": round(tf32_peak, 1), "unit": "TFLOP/s",
@@ -413,7 +424,7 @@ def roofline_from_profile(res, pk, world, per_gpu, hw):
                          "operands, kernel timed inside the step; `achieved` counts ALGORITHMIC FLOPs "
                          "(2*taps*Cin*Cout per pixel) — tf32x3 issues 2 MMAs per product in conv_tc "
                          "(TF32 main + bf16 correction), frac_issued counts both",
-            "traffic": traffic, "traffic_note": traffic_src, "kernels": kern,
+            "kernels": kern,
             "step_tflops_algorithmic": round(step_tflops, 1),
             "step_frac": round(step_tflops / tf32_peak, 3)}
 
@@ -458,7 +469,8 @@ def run_ours(args):
         sampler.start()
     results = {}
     for mth in modes:
-        results[mth] = measure_seg_mode(mth, args, world, rank, dev, (X, y, Xt, yt), gb, per_gpu, hw)
+        results[mth] = measure_seg_mode(mth, args, world, rank, dev, (X, y, Xt, yt), gb, per_gpu, hw,
+                                        args.dump_outputs if mth == modes[0] else None)
     sampler.stop_flag = True
     if rank != 0:
         return
@@ -532,7 +544,11 @@ if __name__ == "__main__":
     ap.add_argument("--ref-batch", type=int, default=BATCH,
                     help="images per step of the CPU arm (default: the full batch of 32)")
     ap.add_argument("--no-baselines", "--no-cpu-baseline", dest="no_baselines", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the losses and trained state of the last timed step as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.dump_outputs and (a.impl != "ours" or a.workload not in ("seg512", "seg256")):
+        ap.error("--dump-outputs writes the Segmentor workloads of our arm (seg512, seg256) only")
     if a.impl == "reference":
         run_reference(a)
     elif a.impl == "torch-cuda":

@@ -1,5 +1,5 @@
 /*
- * atomai_b200.h — C ABI of libatomai_b200.so (sm_100a only).
+ * atomai_b200.h — C ABI of libatomai_b200.so (sm_90a only).
  *
  * Drop-in boundary for the AtomAI data-parallel hot path (SURVEY.md §8b).  The
  * reference (pycroscopy/atomai v0.8.1) has no FFI of its own: every entry point
@@ -11,11 +11,16 @@
  *  - Activations are NHWC fp32 ("pixel-major"): element (n,h,w,c) lives at
  *    ((n*H + h)*W + w)*ld + c, ld >= C (ld lets a tensor be a channel slice).
  *  - Every launch goes to `stream` (a cudaStream_t passed as void*).
+ *  - Sums across CTAs (BatchNorm statistics and backward sums, weight gradients, losses) are
+ *    added in a fixed order, so repeating a call on the same inputs gives bit-identical
+ *    results.  Their partials live in a library-internal device workspace per (device, stream),
+ *    allocated on first use and grown when a larger launch needs it; calls on different streams
+ *    may run concurrently.
  *  - The caller owns every buffer; the library never allocates caller-visible
  *    memory.  Return value: 0 = ok, non-zero = error, text via
  *    atomai_b200_last_error() (thread-local).  No exceptions cross the ABI.
- *  - math: 0 = exact fp32 FFMA kernels, 1 = TF32 tcgen05 tensor-core kernels
- *    (fp32 accumulate in TMEM), 2 = the same kernels with every operand split into
+ *  - math: 0 = exact fp32 FFMA kernels, 1 = TF32 wgmma tensor-core kernels
+ *    (fp32 accumulate in registers), 2 = the same kernels with every operand split into
  *    a TF32 high and low part (three MMAs per product; meets the reference's fp32
  *    results to ~1e-6 relative).  There is no CPU path.
  */
@@ -73,7 +78,7 @@ typedef struct {
 
 const char* atomai_b200_version(void);
 const char* atomai_b200_last_error(void);
-/* 1 if the tcgen05 kernels can run on `device` (compute capability 10.x). */
+/* 1 if the wgmma kernels can run on `device` (compute capability 9.x). */
 int atomai_b200_device_ok(int device);
 
 /* ---- weight preparation -------------------------------------------------
@@ -93,7 +98,7 @@ int atomai_b200_prep_weights(const float* w_oihw, int Cout, int Cin, int ks_h, i
  * :130-132 (UpsampleBlock 1x1), atomai/nets/fcnn.py:115 (px head). */
 int atomai_b200_conv_fwd(const ab_conv_t* d, const float* w_prepped, const float* bias,
                          float* y, int ld_y, double* stats, void* stream);
-/* 1 if the tcgen05 (AB_MATH_TF32) kernel takes this descriptor: which = 0 forward / dgrad
+/* 1 if the tensor-core (AB_MATH_TF32) kernel takes this descriptor: which = 0 forward / dgrad
  * (atomai_b200_conv_fwd), 1 weight gradient (atomai_b200_conv_wgrad).  Callers fall back to
  * AB_MATH_FP32 (exact SIMT kernels) for the rest — thin channel counts, odd strides. */
 int atomai_b200_conv_supported(const ab_conv_t* d, int which);
@@ -244,8 +249,8 @@ int atomai_b200_sqerr_reduce(const float* x, const float* xhat, int64_t n, doubl
  * Dense Gram K[i][j] = os * k(||(x1_i - x2_j) * inv_ls||), kind 0 = RBF,
  * 1 = Matern-2.5 (gpytorch RBFKernel/MaternKernel/ScaleKernel as configured at
  * atomai/nets/gp.py:41-46, :100-111).  x: [n][d] row-major fp32, inv_ls: [d].
- * math: AB_MATH_TF32 / AB_MATH_TF32X3 run the contraction on the tcgen05 convolution kernel
- * with the exponentiation in its TMEM epilogue, AB_MATH_FP32 on exact FFMA tiles.
+ * math: AB_MATH_TF32 / AB_MATH_TF32X3 run the contraction on the tensor-core convolution kernel
+ * with the exponentiation in its register epilogue, AB_MATH_FP32 on exact FFMA tiles.
  * `workspace` (256 B aligned, >= atomai_b200_gram_workspace_bytes) is caller-owned scratch
  * for the scaled/augmented operands; the library allocates nothing. */
 int64_t atomai_b200_gram_workspace_bytes(int n1, int n2, int d);
@@ -307,20 +312,7 @@ int atomai_b200_p2p_bn_finalize(void* const* data_ptrs_host, void* const* flag_p
                                 float* running_var, float momentum, float eps, float* scale,
                                 float* shift, float* mean, float* invstd, void* stream);
 
-/* ---- self-test hooks (tests only) ------------------------------------------------
- * Raw tcgen05 GEMM D[128][N] = A[128][K] B[N][K]^T on core-matrix ("interleave")
- * operands, used by tests to pin descriptor conventions. */
-int atomai_b200_selftest_umma(const float* A, const float* B, float* D, int N, int K,
-                              int variant, void* stream);
-/* tcgen05 issue-rate probe (dev/test only): `issuers` threads each issue `iters` M128 x N x K8 TF32
- * MMAs on resident operands; out[2*i] = SM clocks to issue, out[2*i+1] = clocks until retired.
- * layout 0 = K-major no-swizzle (conv), 1 = MN-major SWIZZLE_128B_BASE32B (wgrad). */
-int atomai_b200_umma_rate(int N, int layout, int issuers, int iters, long long* out, void* stream);
-/* K-major SWIZZLE_128B operand probe (dev only; feasibility of TMA-written activation tiles with
- * tap-shifted starts, DESIGN.md 6.1): D[128][N] = A[128][K] * B[N][K]^T, K in {32, 64};
- * variant bit 0 = halo addressing (8-row groups 18 rows apart), bits 1-3 = row shift. */
-int atomai_b200_selftest_sw128(const float* A, const float* B, float* D, int N, int K,
-                               int variant, void* stream);
+/* ---- self-test hooks (tests only) ------------------------------------------------ */
 /* TMA probe (dev only): one cp.async.bulk.tensor of a {32 ch, TWp, THp, 1} box at (c0, w0, h0, n0)
  * of an NHWC fp32 tensor (out-of-range coordinates are zero-filled) into shared memory at
  * `smem_offset` past a 1024 B boundary, swizzle_mode 0 none / 1 32B / 2 64B / 3 128B /

@@ -9,7 +9,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200, sm_100a)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a)")
 
 
 @pytest.fixture(scope="session")
@@ -18,7 +18,7 @@ def cuda():
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     from atomai_b200 import _C
-    _C.lib()  # fail loudly if the native library is missing on a GPU box
+    _C.lib()  # fail loudly if the native library is missing on a GPU machine
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
     return torch.device("cuda:0")

@@ -73,8 +73,60 @@ def sample_flat(a: np.ndarray, stride: int = 97) -> np.ndarray:
     return np.ascontiguousarray(a.reshape(-1)[::stride])
 
 
+PART_BYTES = 900 * 1024   # every committed fixture file stays below 1 MB
+
+
+class Arrays(OrderedDict):
+    """np.load-like view (`files`, `[key]`) of a fixture stored as several part files."""
+    @property
+    def files(self):
+        return list(self.keys())
+
+
+def save(name: str, **arrays) -> None:
+    """np.savez_compressed into GOLDEN_DIR; a fixture larger than PART_BYTES is written as
+    <stem>.part<i>.npz files of at most PART_BYTES raw bytes each (an array larger than that is cut
+    along axis 0 into '<key>@<j>' pieces, concatenated again by load())."""
+    stem = name[:-len(".npz")]
+    pieces = []
+    for k, v in arrays.items():
+        v = np.asarray(v)
+        if v.nbytes <= PART_BYTES or v.ndim == 0:
+            pieces.append((k, v))
+        else:
+            rows = max(1, PART_BYTES // max(1, v.nbytes // v.shape[0]))
+            pieces += [(f"{k}@{j}", v[i:i + rows]) for j, i in enumerate(range(0, v.shape[0], rows))]
+    if sum(v.nbytes for _, v in pieces) <= PART_BYTES:
+        np.savez_compressed(os.path.join(GOLDEN_DIR, name), **dict(pieces))
+        return
+    parts, cur, size = [], {}, 0
+    for k, v in pieces:
+        if cur and size + v.nbytes > PART_BYTES:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = v
+        size += v.nbytes
+    parts.append(cur)
+    for i, p in enumerate(parts):
+        np.savez_compressed(os.path.join(GOLDEN_DIR, f"{stem}.part{i}.npz"), **p)
+
+
 def load(name: str):
-    return np.load(os.path.join(GOLDEN_DIR, name), allow_pickle=False)
+    path = os.path.join(GOLDEN_DIR, name)
+    if os.path.exists(path):
+        return np.load(path, allow_pickle=False)
+    stem, out, i = name[:-len(".npz")], Arrays(), 0
+    pieces = OrderedDict()
+    while os.path.exists(os.path.join(GOLDEN_DIR, f"{stem}.part{i}.npz")):
+        with np.load(os.path.join(GOLDEN_DIR, f"{stem}.part{i}.npz"), allow_pickle=False) as z:
+            for k in z.files:
+                pieces.setdefault(k.split("@")[0], []).append(z[k])
+        i += 1
+    if not pieces:
+        raise FileNotFoundError(path)
+    for k, v in pieces.items():
+        out[k] = v[0] if len(v) == 1 else np.concatenate(v, 0)
+    return out
 
 
 def subimage_inputs():

@@ -100,7 +100,7 @@ def bfo_case():
     with torch.no_grad():
         logits = net(torch.from_numpy(crop)[None, None]).numpy()
     sd = {k: v.cpu().numpy() for k, v in net.state_dict().items()}
-    np.savez_compressed(os.path.join(HERE, "bfo_weights.npz"), **sd)
+    gu.save("bfo_weights.npz", **sd)
     np.savez_compressed(os.path.join(HERE, "bfo_crop.npz"), image=crop, logits=logits)
     print("bfo", logits.shape, np.abs(logits).max())
 
@@ -120,10 +120,10 @@ def bfo_full_case():
     with torch.no_grad():
         logits = net(torch.from_numpy(x.astype(np.float32))[None, None]).numpy()
     margin = np.sort(np.abs(nn_out[..., :-1].astype(np.float64) - 0.5).reshape(-1))[:16]
-    np.savez_compressed(os.path.join(HERE, "bfo_1024.npz"), image=img,
-                        logits=gu.sample_flat(logits, 61), logits_absmax=np.float64(np.abs(logits).max()),
-                        nn_output=gu.sample_flat(nn_out, 61), coordinates=coords[0],
-                        threshold_margins=margin)
+    gu.save("bfo_1024.npz", image=img,
+            logits=gu.sample_flat(logits, 61), logits_absmax=np.float64(np.abs(logits).max()),
+            nn_output=gu.sample_flat(nn_out, 61), coordinates=coords[0],
+            threshold_margins=margin)
     print("bfo_1024", nn_out.shape, coords[0].shape, "closest |p-0.5|:", margin[:4])
 
 

@@ -19,7 +19,7 @@ def test_library_builds_and_loads():
     path = _C.build()
     assert os.path.exists(path)
     lib = _C.lib()
-    assert b"sm_100a" in lib.atomai_b200_version()
+    assert b"sm_90a" in lib.atomai_b200_version()
 
 
 def test_every_declared_symbol_is_exported_and_bound():

@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 
 FE_CASES = {"fe_37_2": dict(feat=37, embedim=2, n=300, seed=900),
             "fe_64_128": dict(feat=64, embedim=128, n=520, seed=910)}
-# fp32: exact FFMA GEMMs; tf32x3 / tf32: the MLP runs as 1x1 convolutions on tcgen05.
+# fp32: exact FFMA GEMMs; tf32x3 / tf32: the MLP runs as 1x1 convolutions on wgmma.
 # (forward max-rel, gradient rel-L2).  tf32x3 forward: the tensor core accumulates K = 1000 in
 # fp32 with truncation, ~1e-5; tf32 gradients go through three ReLU masks and are only guarded
 # against gross errors (same policy as the TF32 VAE tests).

@@ -100,3 +100,27 @@ def test_predict_coordinates_match_reference_pipeline(cuda):
     assert coords[0].shape == ref_coords.shape
     assert np.abs(coords[0] - ref_coords).max() < 1e-3
     assert np.abs(nn_out - ref_prob).max() < 1e-4
+
+
+def test_training_is_bitwise_reproducible(cuda, tmp_path):
+    """Two fits from the same seed in the default math mode end in bit-identical weights and
+    losses: every cross-CTA reduction of the training path (BatchNorm statistics and backward
+    sums, weight gradients, the loss) adds its partials in a fixed order.  Adam turns last-bit
+    differences of near-zero gradients into full learning-rate steps, so anything less than
+    bitwise equality would show up as visibly different weights."""
+    import atomai_b200 as ab
+    from atomai_b200.models import Segmentor
+    ab.set_math("tf32x3")
+    X, y = _data(16, 128, 128, 21)
+    Xt, yt = _data(8, 128, 128, 23)
+    runs = []
+    for i in range(2):
+        m = Segmentor("Unet", nb_classes=3, seed=1)
+        m.fit(X, y, Xt, yt, training_cycles=5, batch_size=8, filename=str(tmp_path / f"r{i}"),
+              plot_training_history=False)
+        runs.append(({k: v.detach().cpu().clone() for k, v in m.net.state_dict().items()},
+                     [float(v) for v in m.loss_acc["train_loss"] + m.loss_acc["test_loss"]]))
+    (sd0, l0), (sd1, l1) = runs
+    assert l0 == l1
+    for k in sd0:
+        assert torch.equal(sd0[k], sd1[k]), k

@@ -1,6 +1,5 @@
 """Per-layer CUDA-event timing of the three conv kernels (fwd, dgrad, wgrad) on the tensor-core
-layer shapes of the default Unet at the bench workload (batch 32 x 512^2), with the floors of
-profiles/r01_layer_floors.md.  usage: bench_layers.py [fwd] [dgrad] [wgrad] [--math tf32|tf32x3]"""
+layer shapes of the default Unet at the bench workload (batch 32 x 512^2).  usage: bench_layers.py [fwd] [dgrad] [wgrad] [--math tf32|tf32x3]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

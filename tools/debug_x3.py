@@ -1,4 +1,4 @@
-"""Per-kernel accuracy of the tcgen05 paths (tf32 / tf32x3) against float64 on layer shapes."""
+"""Per-kernel accuracy of the tensor-core paths (tf32 / tf32x3) against float64 on layer shapes."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

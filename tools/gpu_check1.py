@@ -1,6 +1,7 @@
-"""Raw-kernel bring-up check on a B200 (dev tool, not a test): every C-ABI kernel against plain
+"""Raw-kernel bring-up check on the GPU (dev tool, not a test): every C-ABI kernel against plain
 torch fp32 ops on the GPU.  Each group runs in its own subprocess so that a trapped kernel cannot
-poison the others.  Usage: python tools/gpu_check1.py [group ...]; writes gpurun_out/check1.json."""
+poison the others.  Usage: python tools/gpu_check1.py [group ...]; prints one JSON line per group
+(and writes them all to $GPU_CHECK1_JSON when that is set)."""
 import json
 import os
 import subprocess
@@ -9,7 +10,7 @@ import traceback
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-GROUPS = ["selftest", "selftest_next", "simt", "tc_basic", "tc_fused", "tc_dgrad", "dgrad_diag", "wgrad_simt", "wgrad_tc",
+GROUPS = ["selftest_tma", "simt", "tc_basic", "tc_fused", "tc_dgrad", "dgrad_diag", "wgrad_simt", "wgrad_tc",
           "elementwise", "vae", "bigshape"]
 
 
@@ -103,52 +104,11 @@ def run_group(name):
         torch.cuda.synchronize()
         res[tag] = {"rel": rel(dw, w.grad)}
 
-    if name == "selftest":
-        for variant in [0, 4] + list(range(8, 24)):
-            for (N, K) in [(64, 32), (32, 8), (128, 64)]:
-                if variant >= 8 or (variant & 2):
-                    At = rnd(K, 128)
-                    Bt = rnd(K, N)
-                    ref = At.t() @ Bt
-                    A_, B_ = At, Bt
-                else:
-                    A = rnd(128, K)
-                    B = rnd(N, K)
-                    ref = A @ B.t()
-                    A_, B_ = A, B
-                D = torch.zeros(128, N, device=dev)
-                try:
-                    ops.selftest_umma(A_.contiguous(), B_.contiguous(), D, N, K, variant)
-                    torch.cuda.synchronize()
-                    res[f"v{variant}_N{N}_K{K}"] = {"rel": rel(D, ref)}
-                except Exception as e:  # noqa
-                    res[f"v{variant}_N{N}_K{K}"] = {"error": str(e)[:200]}
-                    raise
-        for stack in (1, 2, 3):          # stacked-tap A operand (wgrad_tc): A[c*32+i][k] = X[k+c*stack][i]
-            for (N, K) in [(32, 8), (64, 32), (128, 64)]:
-                X = rnd(K + 16, 32)
-                Bt = rnd(K, N)
-                At = torch.cat([X[c * stack:c * stack + K] for c in range(4)], dim=1)   # [K][128]
-                ref = At.t() @ Bt
-                D = torch.zeros(128, N, device=dev)
-                Xin = torch.zeros(128 * K, device=dev)
-                Xin[:X.numel()] = X.reshape(-1)
-                ops.selftest_umma(Xin, Bt.contiguous(), D, N, K, 32 + stack)
-                torch.cuda.synchronize()
-                res[f"stack{stack}_N{N}_K{K}"] = {"rel": rel(D, ref)}
-    elif name == "selftest_next":
-        # feasibility probes for the next round (not asserted by the test-suite): K-major SWIZZLE_128B
-        for variant in [0] + [1 + 2 * sh for sh in range(8)]:
-            for (N, K) in [(32, 32), (64, 64), (128, 64)]:
-                A = rnd(128, K); B = rnd(N, K)
-                D = torch.zeros(128, N, device=dev)
-                ops.selftest_sw128(A.contiguous(), B.contiguous(), D, N, K, variant)
-                torch.cuda.synchronize()
-                res[f"sw128_v{variant}_N{N}_K{K}"] = {"rel": rel(D, A @ B.t())}
+    if name == "selftest_tma":
         # TMA box load of an NHWC halo tile: zero fill outside the image, swizzle = f(absolute address)
         x = rnd(2, 24, 20, 32)
         TWp, THp = 10, 6
-        for mode, chunk, mask in [(0, 16, 0), (3, 16, 7), (4, 32, 3)]:
+        for mode, chunk, mask in [(0, 16, 0), (3, 16, 7)]:
             for off in (0, 128, 384):
                 for (w0, h0) in [(3, 4), (-1, -1), (15, 20)]:
                     out = torch.full((THp * TWp * 32,), float("nan"), device=dev)
@@ -208,6 +168,16 @@ def run_group(name):
         conv_case("dil4", M, 2, 32, 32, [64], 128, dil=4)
         conv_case("dil6", M, 1, 32, 32, [128], 128, dil=6)
         conv_case("nchw_out", M, 2, 32, 32, [32], 32, nchw_out=True, stats=False)
+        # one operand stage per pipeline (n_a = 2, streamed weights, several k-chunks): a plan the
+        # shared-memory budget forces on wide layers; the consumer must hand each stage back
+        # before it waits for the next chunk in the same stage
+        os.environ["ATOMAI_B200_SMEM_KB"], os.environ["ATOMAI_B200_NA4"] = "64", "0"
+        try:
+            for m_, tag in ((M, "one_stage_tf32"), (ops.MATH_TF32X3, "one_stage_tf32x3")):
+                conv_case(tag, m_, 2, 32, 32, [64], 64, affine=True)
+                conv_case(tag + "_pool", m_, 2, 32, 32, [64], 64, pool=True)
+        finally:
+            del os.environ["ATOMAI_B200_SMEM_KB"], os.environ["ATOMAI_B200_NA4"]
     elif name == "tc_dgrad":
         for math, tag in [(ops.MATH_FP32, "simt"), (ops.MATH_TF32, "tc")]:
             for (ci, co, dil) in [(32, 64, 1), (16, 32, 1), (64, 128, 2)]:
@@ -225,7 +195,7 @@ def run_group(name):
                 torch.cuda.synchronize()
                 res[f"{tag}_{ci}_{co}_d{dil}"] = {"rel": rel(nchw(out), x.grad)}
     elif name == "dgrad_diag":
-        # first-launch / shape sensitivity of the tcgen05 path: each case twice, TC vs SIMT
+        # first-launch / shape sensitivity of the tensor-core path: each case twice, TC vs SIMT
         for rep in range(2):
             for (ci, co, dil) in [(32, 64, 1), (64, 32, 1), (32, 64, 1), (16, 32, 1)]:
                 N, H, W = 2, 32, 32
@@ -425,7 +395,6 @@ def main():
         print("@@RESULT@@" + json.dumps(out))
         return
     groups = sys.argv[1:] or GROUPS
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     allres = {}
     for gname in groups:
         try:
@@ -444,8 +413,9 @@ def main():
         except subprocess.TimeoutExpired:
             allres[gname] = {"ok": False, "error": "timeout"}
         print(gname, json.dumps(allres[gname])[:3000], flush=True)
-        with open(os.path.join(ROOT, "gpurun_out", "check1.json"), "w") as f:
-            json.dump(allres, f, indent=1)
+        if os.environ.get("GPU_CHECK1_JSON"):
+            with open(os.environ["GPU_CHECK1_JSON"], "w") as f:
+                json.dump(allres, f, indent=1)
 
 
 if __name__ == "__main__":

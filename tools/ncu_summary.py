@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (ncu --set full) into a small markdown table for profiles/.
+"""Summarise an .ncu-rep (ncu --set full) into a small markdown table.
 usage: ncu_summary.py report.ncu-rep out.md [title]"""
 import csv, io, subprocess, sys
 rep, out = sys.argv[1], sys.argv[2]
