@@ -15,7 +15,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libatomai_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
-           "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu"]
+           "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
+           "segloss.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -101,6 +102,12 @@ SIGNATURES = {
                                      _i64, _i, _vp]),
     "atomai_b200_ce_fwd_bwd": (_i, [_vp, _i, _vp, _i64, _i, _vp, _vp, _i, _f, _vp, _vp]),
     "atomai_b200_pointwise_loss": (_i, [_vp, _vp, _i64, _i, _vp, _vp, _f, _vp, _vp]),
+    "atomai_b200_dice_sums": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "atomai_b200_dice_finalize": (_i, [_vp, _i, _f, _vp, _vp, _vp]),
+    "atomai_b200_dice_bwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _f, _vp, _vp]),
+    "atomai_b200_focal_finalize": (_i, [_vp, _d, _f, _f, _vp, _vp, _vp]),
+    "atomai_b200_iou_hist": (_i, [_vp, _i, _vp, _i, _i64, _i, _i, _f, _vp, _vp]),
+    "atomai_b200_iou_finalize": (_i, [_vp, _i, _vp, _vp]),
     "atomai_b200_adam_multi": (_i, [_vp, _i, _i64, _f, _f, _f, _f, _f, _i, _f, _vp]),
     "atomai_b200_linear_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "atomai_b200_linear_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),

@@ -1,6 +1,9 @@
-from .losses import BCEWithLogitsLoss, CrossEntropyLoss, MSELoss, select_loss
+from .losses import (BCEWithLogitsLoss, CrossEntropyLoss, MSELoss, dice_loss, focal_loss,
+                     select_loss)
+from .metrics import IoU
 from .vi_losses import (infocapacity, kld_normal, kld_rot, reconstruction_loss, rvae_loss,
                         vae_loss)
 
-__all__ = ["select_loss", "CrossEntropyLoss", "BCEWithLogitsLoss", "MSELoss",
-           "reconstruction_loss", "kld_normal", "kld_rot", "vae_loss", "rvae_loss", "infocapacity"]
+__all__ = ["select_loss", "CrossEntropyLoss", "BCEWithLogitsLoss", "MSELoss", "dice_loss",
+           "focal_loss", "IoU", "reconstruction_loss", "kld_normal", "kld_rot", "vae_loss",
+           "rvae_loss", "infocapacity"]

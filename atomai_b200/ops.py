@@ -267,6 +267,52 @@ def pointwise_loss(pred, target, kind, loss_sum, dpred=None, gscale=1.0, gscale_
                                            ptr(gscale_dev), stream_ptr()))
 
 
+def _labels(labels) -> int:
+    """label_float flag of the segmentation objectives (float labels are truncated, int64 read)."""
+    assert labels.is_cuda and labels.is_contiguous() and labels.dtype in (torch.int64, torch.float32)
+    return 1 if labels.dtype == torch.float32 else 0
+
+
+def dice_sums(logits_nhwc, labels, cells) -> None:
+    """cells (float64, 2K) <- per-cell (I, S) sums of the dice loss (K = C*W, or 2 for C == 1)."""
+    N, H, W, Cc = logits_nhwc.shape
+    assert cells.dtype == torch.float64 and cells.is_contiguous() and labels.numel() == N * H * W
+    check(lib().atomai_b200_dice_sums(ptr(logits_nhwc), _ld(logits_nhwc), ptr(labels),
+                                      _labels(labels), N, H, W, Cc, ptr(cells), stream_ptr()))
+
+
+def dice_finalize(cells, eps, loss, coef=None) -> None:
+    check(lib().atomai_b200_dice_finalize(ptr(cells), cells.numel() // 2, float(eps), ptr(loss),
+                                          ptr(coef), stream_ptr()))
+
+
+def dice_bwd(logits_nhwc, labels, coef, dlogits, gscale=1.0, gscale_dev=None) -> None:
+    N, H, W, Cc = logits_nhwc.shape
+    check(lib().atomai_b200_dice_bwd(ptr(logits_nhwc), _ld(logits_nhwc), ptr(labels),
+                                     _labels(labels), N, H, W, Cc, ptr(coef), ptr(dlogits),
+                                     _ld(dlogits), float(gscale), ptr(gscale_dev), stream_ptr()))
+
+
+def focal_finalize(bce_sum, count, alpha, gamma, loss, factor=None) -> None:
+    check(lib().atomai_b200_focal_finalize(ptr(bce_sum), float(count), float(alpha), float(gamma),
+                                           ptr(loss), ptr(factor), stream_ptr()))
+
+
+def iou_hist(logits_nhwc, labels, thresh, counts, activation=True) -> None:
+    """counts (int64, nc*nc, zeroed) += confusion histogram of thresholded predictions vs labels
+    (softmax / sigmoid applied first unless `activation` is false)."""
+    N, H, W, Cc = logits_nhwc.shape
+    assert counts.dtype == torch.int64 and counts.is_contiguous() and labels.numel() == N * H * W
+    check(lib().atomai_b200_iou_hist(ptr(logits_nhwc), _ld(logits_nhwc), ptr(labels),
+                                     _labels(labels), N * H * W, Cc, 1 if activation else 0,
+                                     float(thresh), ptr(counts),
+                                     stream_ptr()))
+
+
+def iou_finalize(counts, nc, out) -> None:
+    check(lib().atomai_b200_iou_finalize(ptr(counts), int(nc), ptr(out), stream_ptr()))
+
+
 def sqerr_reduce(x, xhat, out, dxhat=None, gscale=1.0, gscale_dev=None) -> None:
     check(lib().atomai_b200_sqerr_reduce(ptr(x), ptr(xhat), x.numel(), ptr(out), ptr(dxhat),
                                          float(gscale), ptr(gscale_dev), stream_ptr()))

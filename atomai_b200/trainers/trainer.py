@@ -174,7 +174,7 @@ class BaseTrainer:
             loss = loss / self.comm.world
         if self.compute_accuracy:
             acc_score = self.accuracy_fn(tar, prob)
-            return (loss.item(), acc_score)
+            return (loss.item() if self.sync_host else loss.detach(), acc_score)
         return (loss.item() if self.sync_host else loss.detach(),)
 
     def test_step(self, feat: torch.Tensor, tar: torch.Tensor) -> float:
@@ -191,7 +191,7 @@ class BaseTrainer:
             loss = loss / self.comm.world
         if self.compute_accuracy:
             acc_score = self.accuracy_fn(tar, prob)
-            return (loss.item(), acc_score)
+            return (loss.item() if self.sync_host else loss.detach(), acc_score)
         return (loss.item() if self.sync_host else loss.detach(),)
 
     def _issue_batches(self, e: int):
@@ -284,7 +284,7 @@ class BaseTrainer:
                 loss_ = self.test_step(features_, targets_)
                 running_loss_test += float(loss_[0])
                 if self.compute_accuracy:
-                    running_acc_test += loss_[1]
+                    running_acc_test += float(loss_[1])
                 c += 1
         else:
             for idx in range(len(self.X_test)):
@@ -292,7 +292,7 @@ class BaseTrainer:
                 loss_ = self.test_step(features_, targets_)
                 running_loss_test += float(loss_[0])
                 if self.compute_accuracy:
-                    running_acc_test += loss_[1]
+                    running_acc_test += float(loss_[1])
             c = len(self.X_test)
         if self._is_main():
             print('Model (final state) evaluation loss:', np.around(running_loss_test / c, 4))
@@ -340,9 +340,9 @@ class BaseTrainer:
                'Test loss: {} ...'.format(np.around(float(self.loss_acc["test_loss"][-1]), 4))]
         if self.compute_accuracy:
             msg += ['Train {}: {} ...'.format(
-                        accuracy_metrics, np.around(self.loss_acc["train_accuracy"][-1], 4)),
+                        accuracy_metrics, np.around(float(self.loss_acc["train_accuracy"][-1]), 4)),
                     'Test {}: {} ...'.format(
-                        accuracy_metrics, np.around(self.loss_acc["test_accuracy"][-1], 4))]
+                        accuracy_metrics, np.around(float(self.loss_acc["test_accuracy"][-1]), 4))]
         msg.append('GPU memory usage: {}/{}'.format(gpu_usage[0], gpu_usage[1]))
         print(*msg)
 
@@ -453,6 +453,10 @@ class BaseTrainer:
                 self._bucket.post_scale = 1.0 / self.comm.world
         if self.criterion is None:
             self.criterion = self.get_loss_fn(loss, self.nb_classes)
+        if self.comm is not None and isinstance(self.criterion, (losses_metrics.dice_loss,
+                                                                 losses_metrics.focal_loss)):
+            # not per-pixel means: the loss adds its sums over the ranks before it finalises
+            self.criterion.comm = self.comm
 
         if not self.full_epoch:
             seed = kwargs.get("batch_seed", 1)
@@ -494,7 +498,7 @@ class BaseTrainer:
             if any([e == 0, (e + 1) % self.print_loss == 0, e == self.training_cycles - 1]):
                 self.print_statistics(e)
         if not self.sync_host:   # deferred read-back: one sync at the end instead of one per step
-            for k in ("train_loss", "test_loss"):
+            for k in ("train_loss", "test_loss", "train_accuracy", "test_accuracy"):
                 self.loss_acc[k] = [float(v) for v in self.loss_acc[k]]
         if not self.full_epoch:
             self.eval_model()
@@ -566,9 +570,12 @@ class SegTrainer(BaseTrainer):
                                  " contained in training data")
 
     def accuracy_fn(self, y: torch.Tensor, y_prob: torch.Tensor, *args):
-        raise NotImplementedError(
-            "IoU accuracy (compute_accuracy=True) is a CPU cv2/numpy metric in the reference "
-            "(atomai/losses_metrics/metrics.py:16-95) and outside the accelerated hot path")
+        """Mean IoU of the batch (atomai/trainers/trainer.py:731-737), counted on the GPU; a float
+        per step, or a device scalar read back at the end of the run with sync_host=False.  Under
+        data parallelism the confusion counts are added over the ranks first."""
+        iou = losses_metrics.IoU(y, y_prob, self.nb_classes,
+                                 comm=self.comm if self._world > 1 else None)
+        return iou.evaluate() if self.sync_host else iou.evaluate_device()
 
 
 class ImSpecTrainer(BaseTrainer):

@@ -198,6 +198,39 @@ int atomai_b200_ce_fwd_bwd(const float* logits, int ld, const int64_t* labels, i
 int atomai_b200_pointwise_loss(const float* pred, const float* target, int64_t n, int kind,
                                double* loss_sum, float* dpred, float gscale,
                                const float* gscale_dev, void* stream);
+/* Dice loss (atomai/losses_metrics/losses.py:53-89) over NHWC logits of an N x H x W batch.
+ * C > 1: softmax probabilities, int64 labels (N, H, W); the reference sums over dims (0, 2), so
+ * there are K = C*W cells (class, image column).  C == 1: probabilities [sigmoid, 1 - sigmoid],
+ * targets [y == 1, y == 0] of (N, 1, H, W) labels (float if label_float, else int64), K = 2.
+ * dice_sums writes cells[0:K] = I = sum p*t and cells[K:2K] = S = sum (p + t) (double, ordered
+ * cross-CTA sums, C <= 16, 2*C*ceil(W/32)*32 <= 2^21).  dice_finalize: loss[0] = 1 - mean 2I/(S+eps)
+ * and coef[0:K] = -(2/K)/(S+eps), coef[K:2K] = (2/K) I/(S+eps)^2 (nullable).  dice_bwd:
+ * dlogits = g * dL/dlogits with dL/dp = t*coef[k] + coef[K+k], chained through the softmax /
+ * sigmoid, g = gscale * (gscale_dev ? *gscale_dev : 1). */
+int atomai_b200_dice_sums(const float* logits, int ld, const void* labels, int label_float, int N,
+                          int H, int W, int C, double* cells, void* stream);
+int atomai_b200_dice_finalize(const double* cells, int K, float eps, float* loss, float* coef,
+                              void* stream);
+int atomai_b200_dice_bwd(const float* logits, int ld, const void* labels, int label_float, int N,
+                         int H, int W, int C, const float* coef, float* dlogits, int ld_d,
+                         float gscale, const float* gscale_dev, void* stream);
+/* Focal loss (losses.py:13-50) from the BCE-with-logits sum of atomai_b200_pointwise_loss(kind 1):
+ * CE = *bce_sum / count, pt = exp(-CE), loss[0] = alpha (1-pt)^gamma CE, factor[0] = dloss/dCE
+ * (nullable) — the device scale of the BCE gradient. */
+int atomai_b200_focal_finalize(const double* bce_sum, double count, float alpha, float gamma,
+                               float* loss, float* factor, void* stream);
+
+/* ---- segmentation accuracy -----------------------------------------------------
+ * Mean IoU (atomai/losses_metrics/metrics.py:16-95).  iou_hist: counts[nc*true + pred] += pixels
+ * (int64, nc*nc, caller zeroes; nc = max(C, 2), C <= 64), pred = sum_c c*[softmax_c > thresh]
+ * (0 if above C-1) for C > 1, [sigmoid > thresh] for C == 1 (activation = 0: the raw values
+ * instead of softmax / sigmoid); labels int64 or float
+ * (label_float, truncated); pixels whose label is outside [0, nc) are skipped.
+ * iou_finalize: iou[0] = mean_c diag / (rowsum + colsum - diag + 1e-10) in float32. */
+int atomai_b200_iou_hist(const float* logits, int ld, const void* labels, int label_float,
+                         int64_t npix, int C, int activation, float thresh, int64_t* counts,
+                         void* stream);
+int atomai_b200_iou_finalize(const int64_t* counts, int nc, float* iou, void* stream);
 
 /* ---- optimizer --------------------------------------------------------------
  * torch.optim.Adam step over a table of tensors (trainers/trainer.py:207,539).
