@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "libatomai_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
-           "segloss.cu"]
+           "segloss.cu", "refine.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -27,6 +27,7 @@ MATH_TF32 = 1
 MATH_TF32X3 = 2
 WMODE_FWD = 0
 WMODE_DGRAD = 1
+REFINE_NONFINITE = -2    # AB_REFINE_NONFINITE of include/atomai_b200.h
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -121,6 +122,7 @@ SIGNATURES = {
     "atomai_b200_gram": (_i, [_vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp, _i64, _vp, _i64, _vp]),
     "atomai_b200_prob_mask": (_i, [_vp, _i, _i64, _i, _i, _f, _vp, _i, _vp, _vp]),
     "atomai_b200_gather_windows": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
+    "atomai_b200_peak_refine": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_rowloss": (_i, [_vp, _vp, _i, _i64, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_dropout": (_i, [_vp, _i, _i64, _i, _f, C.c_uint64, _vp, _vp]),
     "atomai_b200_augment": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, C.c_uint64,

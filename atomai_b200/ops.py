@@ -389,6 +389,17 @@ def gather_windows(img_nhwc, table, r: int, out, nanflag=None) -> None:
                                            ptr(out), ptr(nanflag), stream_ptr()))
 
 
+def peak_refine(stack, atoms, dmax: int, popt, info, nfev=None) -> None:
+    """One lmdif fit of a rotated 2-D Gaussian per int32 row (frame, row0, col0, d) of `atoms` to
+    the windows of the fp32 (n, H, W) `stack`: popt (K, 7) float64, info / nfev (K,) int32."""
+    n, h, w = stack.shape
+    assert stack.dtype == torch.float32 and stack.is_contiguous()
+    assert atoms.dtype == torch.int32 and atoms.is_contiguous() and atoms.shape[1:] == (4,)
+    assert popt.dtype == torch.float64 and popt.is_contiguous() and info.dtype == torch.int32
+    check(lib().atomai_b200_peak_refine(ptr(stack), n, h, w, ptr(atoms), atoms.shape[0], int(dmax),
+                                        ptr(popt), ptr(info), ptr(nfev), stream_ptr()))
+
+
 def rowloss(x, xhat, kind: int, out=None, dxhat=None, gvec=None) -> None:
     """Per-sample reconstruction loss over (B, D) rows (kind 0: 0.5*sum sq. err., 1: BCE logits)."""
     B = x.shape[0]

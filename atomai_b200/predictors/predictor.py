@@ -5,7 +5,10 @@ sm_90a graph) and so does the Locator's front end: one kernel turns the NHWC log
 probabilities AND the thresholded binary masks (atomai_b200_prob_mask), batches are copied to
 pinned host buffers asynchronously and synchronised once.  Connected components -> centre of mass
 -> edge filter stay the reference's CPU algorithm (scipy.ndimage) on those masks, bit-exact with
-the reference (tests/golden/locator_crop.npz, bfo_1024.npz).
+the reference (tests/golden/locator_crop.npz, bfo_1024.npz).  With refine=True the Locator then
+fits a 2-D Gaussian around every atom of every frame (atomai/utils/coords.py:179-231): all fits are
+one CUDA launch over the input stack (atomai_b200_peak_refine, MINPACK's lmdif in fp64, one warp per
+atom); the window selection, the default d and the acceptance test stay on the host.
 """
 import time
 from typing import Dict, List, Tuple, Type, Union
@@ -13,7 +16,7 @@ from typing import Dict, List, Tuple, Type, Union
 import numpy as np
 import torch
 
-from ..utils.coords import find_com
+from ..utils.coords import find_com, refine_frames
 from ..utils.img import cv_thresh, img_pad, img_resize
 from ..utils.nn import get_downsample_factor, get_nb_classes, set_train_rng
 from ..utils.preproc import torch_format_image, torch_format_spectra
@@ -262,8 +265,10 @@ class Locator:
     """
     Transforms pixel data from NN output into coordinate data
     (atomai/predictors/predictor.py:531-639): threshold -> 4-connected components -> centre of
-    mass (of the thresholded image) -> drop coordinates within `dist_edge` px of the border.
-    Returns {frame: (n_atoms, 3) float64 [x, y, class]}.
+    mass (of the thresholded image) -> drop coordinates within `dist_edge` px of the border, and
+    with refine=True a 2-D Gaussian fit around each atom in the input images (`run(nn_output,
+    images)`; **d: half-side of the fitted square, default 1/4 of each frame's mean
+    nearest-neighbour distance).  Returns {frame: (n_atoms, 3) float64 [x, y, class]}.
 
     Example:
         >>> coordinates = Locator(dist_edge=10, refine=False).run(nn_output)
@@ -308,9 +313,14 @@ class Locator:
                     (coord_ch, np.zeros((coord_ch.shape[0], 1)) + ch), axis=1))
             d_coord[i] = np.concatenate(per_class, axis=0) if per_class else np.empty((0, 3))
         if self.refine:
-            raise NotImplementedError(
-                "2-D Gaussian peak refinement (atomai/utils/coords.py:179-231) is outside the "
-                "accelerated hot path; pass refine=False")
+            if len(args) == 0:
+                raise AssertionError("Pass input image(s) for coordinates refinement")
+            print('\n\rRefining atomic positions... ', end="")
+            imgdata = args[0][..., 0]
+            nfr = min(len(imgdata), len(d_coord))
+            refined = refine_frames(imgdata[:nfr], [d_coord[i] for i in range(nfr)], self.d)
+            print("Done")
+            return dict(enumerate(refined))
         return d_coord
 
     def rem_edge_coord(self, coordinates: np.ndarray, h: int, w: int) -> np.ndarray:

@@ -1,4 +1,5 @@
-from .coords import find_com, grid2xy, imcoordgrid, remove_edge_coord, transform_coordinates
+from .coords import (find_com, get_nn_distances_, grid2xy, imcoordgrid, peak_refinement,
+                     remove_edge_coord, transform_coordinates)
 from .img import (crop_borders, cv_thresh, extract_random_subimages, extract_subimages,
                   extract_subimages_cuda, get_coord_grid,
                   get_imgstack, imcrop_randcoord, imcrop_randpx, img_pad, img_resize)

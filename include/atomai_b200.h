@@ -302,6 +302,19 @@ int atomai_b200_prob_mask(const float* logits, int ld, int64_t npix, int C, int 
  * extraction of atomai/utils/img.py:138-180, 298-350 as one gather. */
 int atomai_b200_gather_windows(const float* img, int n, int h, int w, int c, const int32_t* table,
                                int K, int r, float* out, int32_t* nanflag, void* stream);
+/* 2-D Gaussian peak refinement (atomai/utils/coords.py:152-231, predictors/predictor.py:609-619):
+ * for each of the K rows {frame, row0, col0, d} of `atoms` (int32, device) one least-squares fit of
+ *   offset + amp exp(-(a (x-xo)^2 + 2 b (x-xo)(y-yo) + c (y-yo)^2))
+ * to the window img[frame, row0:row0+2d, col0:col0+2d] of the fp32 (n, H, W) stack, in fp64, by
+ * MINPACK lmdif as scipy.optimize.curve_fit runs it (start (img[d, d], d, d, 1, 1, 0, 0) in window
+ * coordinates, maxfev 1600).  popt: K x 7 doubles {amp, xo, yo, sigma_x, sigma_y, theta, offset};
+ * info: MINPACK's info (1..8, 0 when (2d)^2 < 7) or one of AB_REFINE_*; nfev (nullable): function
+ * evaluations.  row0 < 0 skips an atom.  Every d must lie in [1, dmax], 1 <= dmax <= 16. */
+#define AB_REFINE_SKIPPED -1   /* row0 < 0: not fitted                                    */
+#define AB_REFINE_NONFINITE -2 /* the window holds a NaN or an infinity                   */
+#define AB_REFINE_BAD_ATOM -3  /* frame or window outside the stack, or d outside [1, dmax] */
+int atomai_b200_peak_refine(const float* img, int n, int H, int W, const int32_t* atoms, int K,
+                            int dmax, double* popt, int32_t* info, int32_t* nfev, void* stream);
 /* Per-sample VAE reconstruction loss (atomai/losses_metrics/vi_losses.py:13-37) over B rows of D
  * elements: kind 0 out[b] += 0.5*sum (xhat-x)^2, kind 1 out[b] += sum BCE-with-logits(xhat, x)
  * (double, nullable, caller zeroes); dxhat (nullable) = gvec[b] * d loss_b / d xhat. */
