@@ -34,6 +34,30 @@ struct ConvSimtParams {
   Ordered red;     // quad-lane / tile kernels: ordered sum of the per-warp statistics
 };
 
+// Run-to-run deterministic end of a 256-thread CTA's reduction of NV partials val(i): the warp sums
+// are added in float in warp order (the in-CTA arithmetic of a shared-memory accumulation), the
+// CTA's totals go to its slot of `group`, and the last CTA of the group adds the slots in order and
+// hands each total to add(i, sum).  s_part: NV * 8 floats of shared memory.
+template <int NV, class Val, class Add>
+__device__ __forceinline__ void cta_slots_finish(const Ordered& red, int group, int nctas, int cta,
+                                                 Val val, Add add, float* s_part, unsigned* s_last) {
+  const int warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const float v = warp_sum(val(i));
+    if ((threadIdx.x & 31) == 0) s_part[warp * NV + i] = v;
+  }
+  __syncthreads();
+  double* slot = ordered_slot(red, group, nctas, cta, NV);
+  for (int i = threadIdx.x; i < NV; i += blockDim.x) {
+    float t = 0.f;
+    for (int w = 0; w < 8; ++w) t += s_part[w * NV + i];
+    slot[i] = t;
+  }
+  ordered_finish(red, group, nctas, NV, threadIdx.x, 256, nctas, [] { __syncthreads(); }, add,
+                 s_last);
+}
+
 __global__ void __launch_bounds__(F_THREADS) conv_simt_fwd_kernel(const ConvSimtParams p) {
   extern __shared__ float sm[];
   const int taps = p.th * p.tw;
@@ -41,7 +65,6 @@ __global__ void __launch_bounds__(F_THREADS) conv_simt_fwd_kernel(const ConvSimt
   const int THp = F_TH + 2 * ph, TWp = F_TW + 2 * pw;
   float* s_in = sm;                             // [F_CIT][THp][TWp]
   float* s_w = sm + F_CIT * THp * TWp;          // [taps][F_CIT][F_COT]
-  __shared__ float s_red[2 * F_COT];
 
   const int tile = blockIdx.x;
   const int tw_i = tile % p.tiles_w;
@@ -118,22 +141,31 @@ __global__ void __launch_bounds__(F_THREADS) conv_simt_fwd_kernel(const ConvSimt
       }
     }
   }
-  if (p.stats) {
-    if (tid < 2 * F_COT) s_red[tid] = 0.f;
-    __syncthreads();
+  if (p.stats) {   // warps 2 cg and 2 cg + 1 hold channel group cg; one slot per CTA, ordered sum
+    __shared__ float s_part[2][F_THREADS / 32][4];   // [sum, square][warp][channel of the group]
+    __shared__ unsigned s_last;
+    const int warp = tid >> 5;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const float a = warp_sum(ssum[k]), b = warp_sum(ssq[k]);
       if ((tid & 31) == 0) {
-        atomicAdd(&s_red[cg * 4 + k], a);
-        atomicAdd(&s_red[F_COT + cg * 4 + k], b);
+        s_part[0][warp][k] = a;
+        s_part[1][warp][k] = b;
       }
     }
     __syncthreads();
-    if (tid < F_COT && co0 + tid < p.Cout) {
-      atomicAdd(p.stats + co0 + tid, (double)s_red[tid]);
-      atomicAdd(p.stats + p.Cout + co0 + tid, (double)s_red[F_COT + tid]);
+    double* slot = ordered_slot(p.red, blockIdx.y, gridDim.x, blockIdx.x, 2 * F_COT);
+    if (tid < 2 * F_COT) {
+      const int kind = tid / F_COT, j = tid % F_COT, g = j >> 2, k = j & 3;
+      slot[tid] = s_part[kind][2 * g][k] + s_part[kind][2 * g + 1][k];   // in float, warp order
     }
+    ordered_finish(p.red, blockIdx.y, gridDim.x, 2 * F_COT, tid, F_THREADS, gridDim.x,
+                   [] { __syncthreads(); },
+                   [&](int i, double v) {
+                     const int co = co0 + i % F_COT;
+                     if (co < p.Cout) p.stats[(i < F_COT ? 0 : p.Cout) + co] += v;
+                   },
+                   &s_last);
   }
 }
 
@@ -145,14 +177,12 @@ __global__ void __launch_bounds__(F_THREADS) conv_simt_fwd_kernel(const ConvSimt
 template <int CO>
 __global__ void __launch_bounds__(256) conv_pix_kernel(const ConvSimtParams p, int vec_in) {
   extern __shared__ float s_w[];                 // [taps][Cin][CO] (zero padded to CO)
-  __shared__ float s_red[2 * CO];
   const int taps = p.th * p.tw, Cin = p.S.Ctot;
   const int c0 = p.c0, nco = min(CO, p.Cout - c0);     // this launch's channel block
   for (int i = threadIdx.x; i < taps * Cin * CO; i += blockDim.x) {
     const int co = i % CO, r = i / CO;
     s_w[i] = co < nco ? __ldg(p.w + (size_t)r * p.Cout + c0 + co) : 0.f;
   }
-  if (threadIdx.x < 2 * CO) s_red[threadIdx.x] = 0.f;
   __syncthreads();
   float bias[CO];
 #pragma unroll
@@ -283,19 +313,15 @@ __global__ void __launch_bounds__(256) conv_pix_kernel(const ConvSimtParams p, i
     }
   }
   if (p.stats) {
-#pragma unroll
-    for (int k = 0; k < CO; ++k) {
-      const float a = warp_sum(ssum[k]), b = warp_sum(ssq[k]);
-      if ((threadIdx.x & 31) == 0) {
-        atomicAdd(&s_red[k], a);
-        atomicAdd(&s_red[CO + k], b);
-      }
-    }
-    __syncthreads();
-    if (threadIdx.x < CO && threadIdx.x < nco) {
-      atomicAdd(p.stats + c0 + threadIdx.x, (double)s_red[threadIdx.x]);
-      atomicAdd(p.stats + p.Cout + c0 + threadIdx.x, (double)s_red[CO + threadIdx.x]);
-    }
+    __shared__ float s_part[8 * 2 * CO];
+    __shared__ unsigned s_last;
+    cta_slots_finish<2 * CO>(p.red, 0, gridDim.x, blockIdx.x,
+                             [&](int i) { return i < CO ? ssum[i] : ssq[i - CO]; },
+                             [&](int i, double v) {
+                               const int k = i % CO;
+                               if (k < nco) p.stats[(i < CO ? 0 : p.Cout) + c0 + k] += v;
+                             },
+                             s_part, &s_last);
   }
 }
 
@@ -307,13 +333,11 @@ template <int CO>
 __global__ void __launch_bounds__(256, 2) conv_c1_kernel(const ConvSimtParams p) {
   __shared__ float4 s_w[9 * CO / 4];            // [tap][co]
   __shared__ float4 s_b[CO / 4];
-  __shared__ float s_red[2 * CO];
   const int c0 = p.c0;                                           // channel block of this launch
   for (int i = threadIdx.x; i < 9 * CO; i += blockDim.x)         // packed [tap][Cin = 1][Cout]
     reinterpret_cast<float*>(s_w)[i] = __ldg(p.w + (size_t)(i / CO) * p.Cout + c0 + (i % CO));
   if (threadIdx.x < CO)
     reinterpret_cast<float*>(s_b)[threadIdx.x] = p.bias ? __ldg(p.bias + c0 + threadIdx.x) : 0.f;
-  if (threadIdx.x < 2 * CO) s_red[threadIdx.x] = 0.f;
   __syncthreads();
   const SrcDev sd = p.S.s[0];
   float sc = 1.f, sh = 0.f;
@@ -393,19 +417,14 @@ __global__ void __launch_bounds__(256, 2) conv_c1_kernel(const ConvSimtParams p)
     }
   }
   if (p.stats) {
-#pragma unroll
-    for (int k = 0; k < CO; ++k) {
-      const float a = warp_sum(ssum[k]), b = warp_sum(ssq[k]);
-      if ((threadIdx.x & 31) == 0) {
-        atomicAdd(&s_red[k], a);
-        atomicAdd(&s_red[CO + k], b);
-      }
-    }
-    __syncthreads();
-    if (threadIdx.x < CO) {
-      atomicAdd(p.stats + c0 + threadIdx.x, (double)s_red[threadIdx.x]);
-      atomicAdd(p.stats + p.Cout + c0 + threadIdx.x, (double)s_red[CO + threadIdx.x]);
-    }
+    __shared__ float s_part[8 * 2 * CO];
+    __shared__ unsigned s_last;
+    cta_slots_finish<2 * CO>(p.red, 0, gridDim.x, blockIdx.x,
+                             [&](int i) { return i < CO ? ssum[i] : ssq[i - CO]; },
+                             [&](int i, double v) {
+                               p.stats[(i < CO ? c0 : p.Cout + c0 - CO) + i] += v;
+                             },
+                             s_part, &s_last);
   }
 }
 
@@ -563,7 +582,10 @@ int launch_conv_c1(const ConvSimtParams& p, cudaStream_t stream) {
   int64_t blocks = (pairs + 255) / 256;
   const int64_t cap = (int64_t)ab_num_sms() * 16;
   if (blocks > cap) blocks = cap;
-  conv_c1_kernel<CO><<<(unsigned)blocks, 256, 0, stream>>>(p);
+  if (blocks < 1) blocks = 1;
+  ConvSimtParams q = p;
+  if (p.stats && ab_ordered_ws(stream, blocks * 2 * CO, 1, &q.red)) return 1;
+  conv_c1_kernel<CO><<<(unsigned)blocks, 256, 0, stream>>>(q);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -681,7 +703,9 @@ int launch_conv_pix(const ConvSimtParams& p, cudaStream_t stream) {
   const int64_t cap = (int64_t)ab_num_sms() * 8;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  conv_pix_kernel<CO><<<(unsigned)blocks, 256, smem, stream>>>(p, vec);
+  ConvSimtParams q = p;
+  if (p.stats && ab_ordered_ws(stream, blocks * 2 * CO, 1, &q.red)) return 1;
+  conv_pix_kernel<CO><<<(unsigned)blocks, 256, smem, stream>>>(q, vec);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -689,7 +713,7 @@ int launch_conv_pix(const ConvSimtParams& p, cudaStream_t stream) {
 // ------------------------------------------------------------------ weight gradient
 // grid: (pixel ranges, taps, co-tiles*ci-tiles).  CTA accumulates dW[co 0..63][ci 0..63] of one
 // tap over its pixel range in registers (thread: 4 co x 4 ci), pixels streamed through smem in
-// slabs of 64, then atomically adds into dW (OIHW).
+// slabs of 64; the pixel ranges of a (tap, tile pair) are added into dW (OIHW) in a fixed order.
 constexpr int G_PX = 64, G_CT = 64, G_THREADS = 256;
 
 struct WgradSimtParams {
@@ -756,23 +780,29 @@ __global__ void __launch_bounds__(G_THREADS) conv_simt_wgrad_kernel(const WgradS
         for (int k = 0; k < 4; ++k) acc[i][k] = fmaf(dv[i], xv[k], acc[i][k]);
     }
   }
+  // this CTA's partial dW[64][64] into its slot; the last range of the (tap, tile pair) adds the
+  // ranges in order
   const int taps = p.th * p.tw;
+  const int group = blockIdx.y * gridDim.z + blockIdx.z;
+  double* slot = ordered_slot(p.red, group, gridDim.x, blockIdx.x, G_CT * G_CT);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int co = co0 + a * 4 + i;
-    if (co >= p.Cout) continue;
+  for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int ci = ci0 + b * 4 + k;
-      if (ci < Cin) atomicAdd(p.dw + ((size_t)co * Cin + ci) * taps + t, acc[i][k]);
-    }
-  }
+    for (int k = 0; k < 4; ++k) slot[(a * 4 + i) * G_CT + b * 4 + k] = acc[i][k];
+  __shared__ unsigned s_last;
+  ordered_finish(p.red, group, gridDim.x, G_CT * G_CT, tid, G_THREADS, gridDim.x,
+                 [] { __syncthreads(); },
+                 [&](int i, double v) {
+                   const int co = co0 + i / G_CT, ci = ci0 + i % G_CT;
+                   if (co < p.Cout && ci < Cin) p.dw[((size_t)co * Cin + ci) * taps + t] += (float)v;
+                 },
+                 &s_last);
 }
 
 // ------------------------------------------------------------------ weight gradient, tiny shapes
 // First layer (Cin = 1) and the pixel-wise head (Cout = nb_classes): the 64 x 64 register tiling
 // above would waste > 95 % of its FMAs, so here every thread walks pixels and keeps the whole
-// CO x CI x TW slice of dW in registers; one warp-shuffle reduction + atomics per CTA at the end.
+// CO x CI x TW slice of dW in registers; warp sums, a fixed-order CTA total and an ordered cross-CTA sum at the end.
 // grid: (pixel ranges, tap rows (ks_h), co-groups * ci-groups).
 // Weight gradient of the same layer: dW[co][0][ty][tx] = sum_p dy[p][co] * x[p + tap].  Thread =
 // two adjacent pixels x CO/2 output channels (blockIdx.y picks the half): the 3 x 4 input patch
@@ -824,19 +854,12 @@ __global__ void __launch_bounds__(256, 2) wgrad_c1_kernel(const WgradSimtParams 
       }
     }
   }
-  __shared__ float s_acc[CH * 9];
-  for (int i = threadIdx.x; i < CH * 9; i += blockDim.x) s_acc[i] = 0.f;
-  __syncthreads();
-#pragma unroll
-  for (int a = 0; a < CH; ++a)
-#pragma unroll
-    for (int t = 0; t < 9; ++t) {
-      const float v = warp_sum(acc[a][t]);
-      if ((threadIdx.x & 31) == 0) atomicAdd(&s_acc[a * 9 + t], v);
-    }
-  __syncthreads();
-  for (int i = threadIdx.x; i < CH * 9; i += blockDim.x)
-    atomicAdd(p.dw + (size_t)(co0 + i / 9) * 9 + i % 9, s_acc[i]);   // OIHW with Cin = 1
+  __shared__ float s_part[8 * CH * 9];
+  __shared__ unsigned s_last;
+  cta_slots_finish<CH * 9>(p.red, blockIdx.y, gridDim.x, blockIdx.x,
+                           [&](int i) { return acc[i / 9][i % 9]; },
+                           [&](int i, double v) { p.dw[(size_t)co0 * 9 + i] += (float)v; },  // OIHW, Cin = 1
+                           s_part, &s_last);
 }
 
 // First-layer weight gradient, tile version (same CTA tile, halo staging and lane mapping as
@@ -948,7 +971,9 @@ int launch_wgrad_c1(const WgradSimtParams& p, cudaStream_t stream) {
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   dim3 grid((unsigned)bx, 2, 1);
-  wgrad_c1_kernel<CO><<<grid, 256, 0, stream>>>(p);
+  WgradSimtParams q = p;
+  if (ab_ordered_ws(stream, bx * 2 * (CO / 2) * 9, 2, &q.red)) return 1;
+  wgrad_c1_kernel<CO><<<grid, 256, 0, stream>>>(q);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -1016,25 +1041,17 @@ __global__ void __launch_bounds__(256) wgrad_small_kernel(const WgradSimtParams 
       }
     }
   }
-  constexpr int NA = CO * CI * TH * TW;
-  __shared__ float s_acc[NA];
-  for (int i = threadIdx.x; i < NA; i += blockDim.x) s_acc[i] = 0.f;
-  __syncthreads();
-#pragma unroll
-  for (int a = 0; a < CO; ++a)
-#pragma unroll
-    for (int b = 0; b < CI; ++b)
-#pragma unroll
-      for (int t = 0; t < TH * TW; ++t) {
-        const float v = warp_sum(acc[a][b][t]);
-        if ((threadIdx.x & 31) == 0) atomicAdd(&s_acc[(a * CI + b) * (TH * TW) + t], v);
-      }
-  __syncthreads();
-  for (int i = threadIdx.x; i < NA; i += blockDim.x) {
-    const int t = i % (TH * TW), b = (i / (TH * TW)) % CI, a = i / (TH * TW * CI);
-    if (co0 + a < p.Cout && ci0 + b < Cin)
-      atomicAdd(p.dw + ((size_t)(co0 + a) * Cin + ci0 + b) * (TH * TW) + t, s_acc[i]);
-  }
+  constexpr int NA = CO * CI * TH * TW, T = TH * TW;
+  __shared__ float s_part[8 * NA];
+  __shared__ unsigned s_last;
+  cta_slots_finish<NA>(p.red, blockIdx.z, gridDim.x, blockIdx.x,
+                        [&](int i) { return acc[i / (T * CI)][(i / T) % CI][i % T]; },
+                        [&](int i, double v) {
+                          const int t = i % T, b = (i / T) % CI, a = i / (T * CI);
+                          if (co0 + a < p.Cout && ci0 + b < Cin)
+                            p.dw[((size_t)(co0 + a) * Cin + ci0 + b) * T + t] += (float)v;
+                        },
+                        s_part, &s_last);
 }
 
 // Weight gradient of a pixel-wise head with <= 4 outputs from 16 input channels (16 -> nb_classes,
@@ -1109,7 +1126,9 @@ int launch_wgrad_small(const WgradSimtParams& p, cudaStream_t stream) {
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
   dim3 grid((unsigned)bx, 1, co_groups * ci_groups);
-  wgrad_small_kernel<CO, CI, TH, TW><<<grid, 256, 0, stream>>>(p, co_groups);
+  WgradSimtParams q = p;
+  if (ab_ordered_ws(stream, bx * grid.z * (CO * CI * TH * TW), grid.z, &q.red)) return 1;
+  wgrad_small_kernel<CO, CI, TH, TW><<<grid, 256, 0, stream>>>(q, co_groups);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -1202,6 +1221,7 @@ int ab_conv_simt_fwd(const ab_conv_t* d, const float* w, const float* bias, floa
   AB_CHECK(tiles < (1ll << 31), "conv_simt: too many tiles");
   if (tiles == 0) return 0;
   dim3 grid((unsigned)tiles, (d->Cout + F_COT - 1) / F_COT);
+  if (stats && ab_ordered_ws(stream, tiles * grid.y * 2 * F_COT, grid.y, &p.red)) return 1;
   conv_simt_fwd_kernel<<<grid, F_THREADS, smem, stream>>>(p);
   AB_LAUNCH_CHECK();
   return 0;
@@ -1244,6 +1264,8 @@ int ab_conv_simt_wgrad(const ab_conv_t* d, const float* dy, int ld_dy, float* dw
   ranges = (p.npix + ppc - 1) / ppc;
   p.px_per_cta = (int)ppc;
   dim3 grid((unsigned)ranges, taps, p.co_tiles * p.ci_tiles);
+  if (ab_ordered_ws(stream, (int64_t)ranges * grid.y * grid.z * G_CT * G_CT, grid.y * grid.z, &p.red))
+    return 1;
   conv_simt_wgrad_kernel<<<grid, G_THREADS, 0, stream>>>(p);
   AB_LAUNCH_CHECK();
   return 0;

@@ -21,8 +21,12 @@
  *    atomai_b200_last_error() (thread-local).  No exceptions cross the ABI.
  *  - math: 0 = exact fp32 FFMA kernels, 1 = TF32 wgmma tensor-core kernels
  *    (fp32 accumulate in registers), 2 = the same kernels with every operand split into
- *    a TF32 high and low part (three MMAs per product; meets the reference's fp32
- *    results to ~1e-6 relative).  There is no CPU path.
+ *    hi = rn_tf32(v) and lo = v - hi.  Forward / data gradient: per k-step one TF32 MMA on
+ *    (a_hi, w_hi) plus one bf16 MMA that adds a_lo*w + a_hi*w_lo; weight gradient: three TF32
+ *    MMAs (hi, hi), (lo, hi), (hi, lo).  lo*lo is not formed.  Per element,
+ *    |y - y_exact| <= (2^-18 + (K+2) 2^-23) * (sum |x||w| + |b|) for K = taps * Cin (pixels
+ *    for the weight gradient), against 2^-10 + (K+2) 2^-23 in mode 1 and (K+2) 2^-24 in
+ *    mode 0 (tests/test_conv_exact_gpu.py).  There is no CPU path.
  */
 #ifndef ATOMAI_B200_H
 #define ATOMAI_B200_H
@@ -35,7 +39,7 @@ extern "C" {
 
 #define AB_MATH_FP32 0
 #define AB_MATH_TF32 1
-#define AB_MATH_TF32X3 2 /* 3xTF32 split: a_hi*w_hi + a_lo*w_hi + a_hi*w_lo, ~fp32 accuracy */
+#define AB_MATH_TF32X3 2 /* split operands: a_hi*w_hi + a_lo*w + a_hi*w_lo (see `math` above) */
 
 #define AB_ACT_LRELU 0
 #define AB_ACT_TANH 1
@@ -92,7 +96,7 @@ int atomai_b200_prep_weights(const float* w_oihw, int Cout, int Cin, int ks_h, i
 
 /* ---- convolution forward (also used for dgrad with AB_WMODE_DGRAD weights) --
  * y = lrelu(conv(x) + bias); optional per-channel (sum, sum^2) of y into
- * stats[2*Cout] (double, accumulated with atomics; caller zeroes).
+ * stats[2*Cout] (double, caller zeroes; added to in a fixed order, see Conventions).
  * Replaces nn.Conv2d + nn.LeakyReLU (+ the statistics pass of nn.BatchNorm2d):
  * atomai/nets/blocks.py:61-76 (ConvBlock), :302-319 (DilatedBlock),
  * :130-132 (UpsampleBlock 1x1), atomai/nets/fcnn.py:115 (px head). */

@@ -4,7 +4,6 @@ in every math mode and under the plan knobs.  Runs without a GPU (the plan is ho
 descriptor carries fake, aligned device pointers that are never dereferenced)."""
 import ctypes as C
 import itertools
-import os
 
 import pytest
 
@@ -67,3 +66,58 @@ def test_plan_knobs_keep_every_unet_layer_plannable(env, monkeypatch):
         for hw in (32, 512):
             rc, _, _, smem = info(make_desc(cins, hw, cout, ks, 1, pool, ops.MATH_TF32X3))
             assert rc == 0 and smem <= OPT_IN, (env, cins, cout, smem)
+
+
+def layer_desc(layer, math):
+    """Descriptor of a tests/test_conv_exact_gpu.py Layer on fake, aligned device pointers."""
+    d = _C.Conv()
+    d.N, d.H, d.W, d.Cout = layer.N, layer.H, layer.W, layer.cout
+    d.ks_h, d.ks_w, d.dil = layer.ks[0], layer.ks[1], layer.dil
+    d.nsrc = len(layer.srcs)
+    for i, s in enumerate(layer.srcs):
+        e = d.src[i]
+        e.ptr = 0x10000000 * (i + 1)
+        e.scale = e.shift = None
+        e.C, e.ld, e.pool = s.C, s.C + s.pad, s.tr
+    d.lrelu, d.math, d.out_nchw, d.act = 1.0, math, 0, ops.ACT_LRELU
+    return d
+
+
+def test_exact_suite_plan_matrix_covers_every_variant(monkeypatch, capfd):
+    """Each forced entry of the exact GPU suite's plan matrix still gets the plan it names, and
+    together they cover every conv_tc plan variant and consumer instantiation.  If the plan
+    heuristics change, this fails here instead of silently moving GPU coverage.  The plan never
+    gives a streamed layer fewer than two weight stages per pipeline (n_b >= 4), so the smallest
+    weight ring it can produce, n_b = 4, stands in for the one-stage ring."""
+    from test_conv_exact_gpu import PLAN_MATRIX, launch_widths, parse_plan
+    monkeypatch.setenv("ATOMAI_B200_PLAN_LOG", "1")
+    seen = []
+    for tag, env, layer, math, want in PLAN_MATRIX:
+        with monkeypatch.context() as mp:
+            for k, v in env.items():
+                mp.setenv(k, v)
+            capfd.readouterr()
+            rc, _, _, smem = info(layer_desc(layer, math))
+            text = capfd.readouterr().err
+        assert rc == 0, (tag, _C.lib().atomai_b200_last_error())
+        assert 0 < smem <= OPT_IN, (tag, smem)
+        got = parse_plan(text)
+        assert got == want, f"{tag}: plan {got}, the matrix expects {want}"
+        seen.append((got, layer))
+    plans = [p for p, _ in seen]
+    assert any(p["resident"] for p in plans)
+    assert any(not p["resident"] and p["sub"] == 1 for p in plans)
+    assert any(not p["resident"] and p["sub"] == 2 for p in plans)
+    assert {p["KC"] for p in plans} == {8, 16, 32}
+    assert {p["n_a"] for p in plans} == {2, 4}
+    assert any(p["n_a"] == 2 and p["resident"] for p in plans)
+    assert any(p["n_a"] == 2 and not p["resident"] for p in plans)
+    assert any(p["n_b"] == 4 for p in plans)
+    assert {p["tma"] for p in plans} == {0, 1}
+    assert any(p["tma"] and p["KC"] == 8 for p in plans)
+    consumers = {(nn, p["sub"]) for p, layer in seen for nn in launch_widths(layer.cout)}
+    every = {(nn, 1) for nn in range(16, 129, 16)} | {(nn, 2) for nn in range(16, 65, 16)}
+    assert consumers == every, f"missing consumer instantiations: {sorted(every - consumers)}"
+    assert any(len(launch_widths(layer.cout)) > 1 for _, layer in seen)
+    assert any(len(layer.srcs) == 2 and layer.srcs[0].C % p["KC"] for p, layer in seen), \
+        "no concat whose split falls inside a k-chunk"

@@ -2,6 +2,10 @@
 ops on the same GPU: every export of include/atomai_b200.h the hot path uses, in both math modes,
 plus size-independent properties at the BASELINE.json workload size (32 x 512 x 512).
 
+tests/test_conv_exact_gpu.py pins the convolution kernels much tighter: bit-exact against float64
+on exactly representable data in every math mode and tile plan, and per element against the
+rounding model on normal data.  The comparisons here stay as a second, independent reference.
+
 The case library lives in tools/gpu_check1.py (also used for bring-up on the box); thresholds:
   fp32 (exact FFMA kernels)   rel = max|a-ref|/max|ref| <= 5e-6, BN statistics 1e-6
   tf32 (wgmma)                rel <= 1e-3 (TF32 operand rounding, measured 2.6-4.2e-4), stats 5e-4
