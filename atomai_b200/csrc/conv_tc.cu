@@ -1,12 +1,15 @@
 // conv_tc.cu — implicit-GEMM convolution on the Hopper tensor cores (wgmma, TF32 operands, fp32
-// accumulators in registers).  One persistent, warp-specialised CTA per SM:
+// accumulators in registers).  One persistent, warp-specialised CTA per SM, two pipelines that
+// work on alternate tiles, each with its own consumer and loader warpgroup:
 //
-//   warps 0-3   consumer   wgmma for every (k-chunk, tap, k-step) of a tile, then the epilogue from
-//                          the accumulator registers: bias + activation -> NHWC/NCHW store + BN statistics
-//   warps 5, 7  producers  cp.async.bulk of pre-packed weight blobs (L2 -> smem), TMA activation tiles
-//   warps 8-15  loaders    HBM/L2 -> regs -> [BN affine, 2x2 max-pool, zero pad, RN->TF32] -> smem
-//                          (two groups of 4 warps = two pipelines working on alternate tiles;
-//                          setmaxnreg moves registers from the producer warpgroup to the others)
+//   warps 0-3, 4-7    consumer g   wgmma for every (k-chunk, tap, k-step) of pipeline g's tiles, then
+//                                  the epilogue from the accumulator registers: bias + activation ->
+//                                  NHWC/NCHW store + BN statistics; refills its own weight ring
+//                                  (streamed weights) with cp.async.bulk of the pre-packed blob
+//   warps 8-11, 12-15 loaders g    HBM/L2 (or a TMA-staged raw tile) -> regs -> [BN affine, 2x2
+//                                  max-pool, zero pad, RN->TF32] -> smem for pipeline g
+//
+// While one consumer waits for a stage or runs its epilogue, the other keeps the tensor core fed.
 //
 // GEMM view (SURVEY.md §8a): M = 64 output pixels (an 8 x 8 tile = one m64 wgmma row block, or
 // 8 x 16 as two sub-tiles when N <= 64), N = Cout (<= 128 per launch; wider layers run one launch
@@ -25,6 +28,7 @@
 
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -32,19 +36,19 @@ namespace {
 
 constexpr int kTileH = 8;
 constexpr int kTileW = 8;
-constexpr int kNumEpiWarps = 4;     // the consumer warpgroup
-constexpr int kWgtWarp = 5;
-constexpr int kWgtWarp2 = 7;        // second weight / TMA producer (pipeline 1)
-constexpr int kFirstLoadWarp = 8;
+constexpr int kNumEpiWarps = 4;     // warps per consumer warpgroup
+constexpr int kNumConsWarps = 2 * kNumEpiWarps;
+constexpr int kFirstLoadWarp = kNumConsWarps;
 constexpr int kNumLoadWarps = 8;
 constexpr int kThreads = (kFirstLoadWarp + kNumLoadWarps) * 32;
-constexpr int kEpiBWarp = kThreads / 32;
-// register re-balancing between the warpgroups (sum * 128 threads = 64K registers).  ptxas still
-// allocates every branch for the 512-thread launch bound (128 registers per thread), so these
-// values only move the physical registers; the consumer's SUB * N / 2 <= 64 fp32 accumulators are
-// what fits that bound (the epilogue spills some of its temporaries to the stack)
-constexpr int kRegsEpi = 232, kRegsMma = 40, kRegsLoad = 120;
-static_assert(kRegsEpi + kRegsMma + 2 * kRegsLoad <= 512, "register budget");
+// register split between the warpgroups (2 * (consumer + loader) * 128 threads = 64K registers).
+// The kernel is launched at 128 registers per thread and setmaxnreg moves them between the
+// warpgroups.  The loaders keep 120 (their U <= kMaxU staged float4s); the consumers get the
+// rest, 136.  More does not help them: with CUDA 12.9 ptxas kept the consumer code within about
+// 136 registers even when setmaxnreg allowed 160 or 232, and those splits only made the kernel's
+// stack frame larger.
+constexpr int kRegsCons = 136, kRegsLoad = 120;
+static_assert(2 * (kRegsCons + kRegsLoad) <= 512, "register budget");
 constexpr int kMaxN = 128;          // output channels per launch (accumulator registers)
 constexpr int kMaxAStages = 4;
 constexpr int kMaxBStages = 32;     // streamed weights: bytes in flight must cover the L2 latency
@@ -92,7 +96,7 @@ struct ConvTcParams {
 
 struct __align__(8) SharedCtl {
   uint64_t full_a[kMaxAStages], empty_a[kMaxAStages];
-  uint64_t full_b[kMaxBStages], empty_b[kMaxBStages];
+  uint64_t full_b[kMaxBStages];
   uint64_t raw_full[kMaxRStages], raw_empty[kMaxRStages];
   uint64_t w_full;
   unsigned red_last;
@@ -106,17 +110,49 @@ __device__ __forceinline__ void consumer_release(uint32_t bar) {
   }
 }
 
-// The consumer warpgroup's whole tile loop, specialised on (N = output channels of this launch,
-// 8-pixel sub-tiles).  Tiles alternate between the two pipelines (loader group / weight ring i
-// stages the tiles with local index = i mod 2).  A k-chunk (resident weights) or a tap (streamed
-// weights) is one wgmma group; a stage is handed back to its producer when the group after its
+// named barriers (id 0 = __syncthreads, 1 = the consumers' final statistics sum)
+constexpr int kStatBar = 2;   // 2..5: consumer 0 -> 1 statistics token of warp w, 6..9: 1 -> 0
+__device__ __forceinline__ void named_bar_sync(int id, int n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int n) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+
+// Streamed-weight refill issued by one thread of a consumer warpgroup.  The copies are predicated
+// instead of branched on: a divergent branch while MMAs are in flight makes ptxas serialise them.
+__device__ __forceinline__ void expect_tx_if(uint32_t pred, uint32_t bar, uint32_t bytes) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %0, 0;\n\t"
+      "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%1], %2;\n\t}" ::"r"(pred), "r"(bar), "r"(bytes)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_g2s_if(uint32_t pred, uint32_t dst_smem, const void* src,
+                                            uint32_t bytes, uint32_t bar) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %0, 0;\n\t"
+      "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%1], [%2], %3, [%4];\n\t}" ::
+          "r"(pred), "r"(dst_smem), "l"(src), "r"(bytes), "r"(bar)
+      : "memory");
+}
+
+// The tile loop of consumer warpgroup `pipe`, specialised on (N = output channels of this launch,
+// 8-pixel sub-tiles).  Consumer g owns the tiles with CTA-local index = g (mod 2), the operand
+// ring half g (filled by loader group g) and the weight ring half g.  A k-chunk (resident weights)
+// or a tap (streamed weights) is one wgmma group; a stage is handed back when the group after its
 // last use has been issued and the one using it has retired (wgmma.wait_group 1), so the tensor
-// core always has the next group queued.
-template <int N, int SUB>
+// core always has the next group queued.  A streamed weight stage is refilled at that point by
+// the consumer's first thread with the piece it holds next (n_b/2 pieces ahead): the retired group
+// was issued by all four warps, so none of them still waits for the stage's previous contents.
+template <int N, int SUB, int PIPE>
 __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* ctl, uint32_t a_base,
                                               uint32_t b_base, float* s_stats, const float* s_bias) {
+  // PIPE is a template parameter: control flow that depends on the thread index puts the MMAs on
+  // a divergent path for ptxas, which then serialises them (C7520)
+  constexpr int pipe = PIPE;
   constexpr int R = N / 2;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = (threadIdx.x >> 5) & (kNumEpiWarps - 1), lane = threadIdx.x & 31;
+  const uint32_t leader = (threadIdx.x & (kNumEpiWarps * 32 - 1)) == 0 ? 1u : 0u;
   const uint32_t ring_n = p.n_a / 2, nb2 = p.n_b / 2;
   const int ksteps = p.KC >> 3;
   const int th = p.taps_h, tw = p.taps_w, taps = th * tw;
@@ -129,20 +165,45 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
   const uint64_t b_tmpl = wgmma_desc(0, p.Cout * 16, 128);
   const uint32_t mb_off = 8u * p.TWp * 16, sb_off = kTileW * 16;
   const uint32_t bar_full_a = smem_u32(&ctl->full_a[0]), bar_empty_a = smem_u32(&ctl->empty_a[0]);
-  const uint32_t bar_full_b = smem_u32(&ctl->full_b[0]), bar_empty_b = smem_u32(&ctl->empty_b[0]);
+  const uint32_t bar_full_b = smem_u32(&ctl->full_b[0]);
   const int tpi = p.tiles_w * p.tiles_h;
   const bool fast = p.act == AB_ACT_LRELU && p.alpha >= 0.f && p.alpha <= 1.f;
   const float alpha = p.alpha;
   float* my_stats = s_stats + warp * 2 * p.Cout;
-  if (res) mbar_wait_quiet(smem_u32(&ctl->w_full), 0);
-  uint32_t sa0 = 0, pa0 = 0, sb0 = 0, pb0 = 0, sa1 = 0, pa1 = 0, sb1 = 0, pb1 = 0;
+  const int tile_step = 2 * gridDim.x;
+  const uint32_t ring0 = pipe * ring_n, b_ring0 = pipe * nb2;
+  uint32_t s_a = 0, p_a = 0, s_b = 0, p_b = 0;
+  // streamed weights: copy the piece `ahead` pieces after (r_tile, r_ch, r_t) of this consumer's
+  // sequence into weight stage `stage`
+  auto refill_b = [&](uint32_t stage, int r_tile, int r_ch, int r_t, int ahead) {
+    r_t += ahead;
+    while (r_t >= taps) {
+      r_t -= taps;
+      if (++r_ch == p.n_chunks) { r_ch = 0; r_tile += tile_step; }
+    }
+    if (r_tile < p.num_tiles) {
+      // piece (k-step s, kind, tap) of the blob lives at ((s*wmult + kind)*taps + tap); the stage
+      // holds [k-step][kind] pieces
+      const uint32_t bar = bar_full_b + (b_ring0 + stage) * 8;
+      expect_tx_if(leader, bar, p.b_stage_bytes);
+      for (int ks = 0; ks < ksteps; ++ks)
+        for (uint32_t kd = 0; kd < wmult; ++kd)
+          bulk_g2s_if(leader, b_base + (b_ring0 + stage) * p.b_stage_bytes + (ks * wmult + kd) * piece,
+                      p.wblob + ((((size_t)r_ch * ksteps + ks) * wmult + kd) * taps + r_t) * (piece >> 2),
+                      piece, bar);
+    }
+  };
+  if (res) {
+    mbar_wait_quiet(smem_u32(&ctl->w_full), 0);
+  } else {
+    for (uint32_t i = 0; i < nb2; ++i) refill_b(i, blockIdx.x + pipe * gridDim.x, 0, 0, (int)i);
+  }
   constexpr int MB = kTileH / 8;               // m64 row blocks per sub-tile
   float acc[SUB][MB][R];
 
-  auto tile_fn = [&](const int tile, const int pipe, uint32_t& s_a, uint32_t& p_a, uint32_t& s_b,
-                     uint32_t& p_b) {
-    const uint32_t ring0 = pipe * ring_n, b_ring0 = pipe * nb2;
-    uint32_t pend_a = 0, pend_b = 0, accum = 0;
+  auto tile_fn = [&](const int tile) {
+    uint32_t pend_a = 0, accum = 0;
+    bool pend_b = false;
     for (int ch = 0; ch < p.n_chunks; ++ch) {
       if (pend_a && ring_n == 1) {
         // one operand stage per pipeline: the stage this chunk needs is the one still held for
@@ -159,8 +220,8 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
         if (!res) {
           if (pend_b && nb2 == 1) {   // the same for a one-stage weight ring
             wgmma_wait<0>();
-            consumer_release(pend_b);
-            pend_b = 0;
+            refill_b((s_b + nb2 - 1) % nb2, tile, ch, t, (int)nb2 - 1);
+            pend_b = false;
           }
           mbar_wait_quiet(bar_full_b + (b_ring0 + s_b) * 8, p_b);
           b_stage = b_base + (b_ring0 + s_b) * p.b_stage_bytes;
@@ -194,11 +255,11 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
         wgmma_commit();
         wgmma_wait<1>();
         consumer_release(pend_a);
-        consumer_release(pend_b);
+        if (pend_b) refill_b((s_b + nb2 - 1) % nb2, tile, ch, t, (int)nb2 - 1);
         pend_a = 0;
-        pend_b = 0;
+        pend_b = false;
         if (!res) {
-          pend_b = bar_empty_b + (b_ring0 + s_b) * 8;
+          pend_b = true;
           if (++s_b == nb2) { s_b = 0; p_b ^= 1; }
         }
         if (t == taps - 1) {
@@ -213,88 +274,115 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
 #pragma unroll
       for (int mb = 0; mb < MB; ++mb) wgmma_fence_regs(acc[s][mb]);
     consumer_release(pend_a);
-    consumer_release(pend_b);
+    if (pend_b) refill_b((s_b + nb2 - 1) % nb2, tile + tile_step, 0, 0, (int)nb2 - 1);
 
     // ---------------- epilogue: registers -> bias + activation -> global store + BN statistics
     const int n = tile / tpi, rem = tile - n * tpi;
     const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
     const int c_lane = 2 * (lane & 3);
+    // this tile's channel sums, added once the token arrives.  After the butterfly every lane of
+    // a channel pair holds the same sums, so column group j is kept by the lanes with
+    // lane >> 2 == j % 8 only: R / 32 groups per lane instead of R / 4
+    constexpr int JL = (R / 4 + 7) / 8;
+    float st[JL][4];
+    // compiled once for the plain LeakyReLU and once for every other activation: the per-element
+    // activation switch of the general case, unrolled over the tile, is what the epilogue spilled
+    auto epilogue = [&](auto fast_tag) {
+      constexpr bool FAST = decltype(fast_tag)::value;
 #pragma unroll
-    for (int j = 0; j < R / 4; ++j) {
-      const int cl = 8 * j + c_lane;              // column within this launch
-      const int c = p.n0 + cl;
-      const float b0 = s_bias[c], b1 = s_bias[c + 1];
-      float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+      for (int j = 0; j < R / 4; ++j) {
+        const int cl = 8 * j + c_lane;              // column within this launch
+        const int c = p.n0 + cl;
+        const float b0 = s_bias[c], b1 = s_bias[c + 1];
+        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
 #pragma unroll
-      for (int s = 0; s < SUB; ++s)
+        for (int s = 0; s < SUB; ++s)
 #pragma unroll
-        for (int mb = 0; mb < MB; ++mb)
+          for (int mb = 0; mb < MB; ++mb)
 #pragma unroll
-          for (int hrow = 0; hrow < 2; ++hrow) {
-            const int gh = th_i * kTileH + mb * 8 + 2 * warp + hrow;
-            const int gw = (tw_i * SUB + s) * kTileW + (lane >> 2);
-            const bool valid = gh < p.H && gw < p.W;
-            float v0 = acc[s][mb][4 * j + 2 * hrow] + b0, v1 = acc[s][mb][4 * j + 2 * hrow + 1] + b1;
-            if (fast) {
-              v0 = fmaxf(v0, v0 * alpha);
-              v1 = fmaxf(v1, v1 * alpha);
-            } else if (p.act == AB_ACT_RBF) {     // alpha * exp(-x/2) as one FMUL + EX2
-              v0 = alpha * exp2f(-0.72134752f * fmaxf(v0, 0.f));
-              v1 = alpha * exp2f(-0.72134752f * fmaxf(v1, 0.f));
-            } else {
-              v0 = act_f(v0, p.act, alpha);
-              v1 = act_f(v1, p.act, alpha);
-            }
-            v0 = valid ? v0 : 0.f;
-            v1 = valid ? v1 : 0.f;
-            if (valid) {
-              const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
-              if (!p.out_nchw) {
-                *reinterpret_cast<float2*>(p.out + pix * p.ld_out + c) = make_float2(v0, v1);
+            for (int hrow = 0; hrow < 2; ++hrow) {
+              const int gh = th_i * kTileH + mb * 8 + 2 * warp + hrow;
+              const int gw = (tw_i * SUB + s) * kTileW + (lane >> 2);
+              const bool valid = gh < p.H && gw < p.W;
+              float v0 = acc[s][mb][4 * j + 2 * hrow] + b0, v1 = acc[s][mb][4 * j + 2 * hrow + 1] + b1;
+              if (FAST) {
+                v0 = fmaxf(v0, v0 * alpha);
+                v1 = fmaxf(v1, v1 * alpha);
+              } else if (p.act == AB_ACT_RBF) {     // alpha * exp(-x/2) as one FMUL + EX2
+                v0 = alpha * exp2f(-0.72134752f * fmaxf(v0, 0.f));
+                v1 = alpha * exp2f(-0.72134752f * fmaxf(v1, 0.f));
               } else {
-                const size_t hw = (size_t)p.nchw_stride;
-                float* o = p.out + ((size_t)n * p.Cout + c) * hw + (size_t)gh * p.W + gw;
-                o[0] = v0;
-                o[hw] = v1;
+                v0 = act_f(v0, p.act, alpha);
+                v1 = act_f(v1, p.act, alpha);
               }
+              v0 = valid ? v0 : 0.f;
+              v1 = valid ? v1 : 0.f;
+              if (valid) {
+                const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
+                if (!p.out_nchw) {
+                  *reinterpret_cast<float2*>(p.out + pix * p.ld_out + c) = make_float2(v0, v1);
+                } else {
+                  const size_t hw = (size_t)p.nchw_stride;
+                  float* o = p.out + ((size_t)n * p.Cout + c) * hw + (size_t)gh * p.W + gw;
+                  o[0] = v0;
+                  o[hw] = v1;
+                }
+              }
+              s0 += v0; s1 += v1;
+              q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
             }
-            s0 += v0; s1 += v1;
-            q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
-          }
-      if (p.stats) {   // the 8 lanes sharing (lane & 3) hold the same two channels
+        if (p.stats) {   // the 8 lanes sharing (lane & 3) hold the same two channels
 #pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-          s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-          q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-          q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-        }
-        if (lane < 4) {
-          my_stats[c] += s0;
-          my_stats[c + 1] += s1;
-          my_stats[p.Cout + c] += q0;
-          my_stats[p.Cout + c + 1] += q1;
+          for (int o = 4; o < 32; o <<= 1) {
+            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+            q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+            q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+          }
+          if ((lane >> 2) == (j & 7)) {
+            st[j >> 3][0] = s0; st[j >> 3][1] = s1; st[j >> 3][2] = q0; st[j >> 3][3] = q1;
+          }
         }
       }
+    };
+    if (fast) epilogue(std::true_type{});
+    else epilogue(std::false_type{});
+    if (p.stats) {
+      // warp w of both consumers adds into s_stats[w] in tile order, as one consumer did: wait
+      // for the other consumer's previous tile, add, pass the token on.  The token is a named
+      // barrier of the two warps (bar.arrive by the passing warp, bar.sync by the waiting one): a
+      // spin on shared memory here puts the next tile's MMAs on a divergent path for ptxas
+      if (tile != (int)blockIdx.x) named_bar_sync(kStatBar + (PIPE ? 0 : kNumEpiWarps) + warp, 64);
+#pragma unroll
+      for (int jl = 0; jl < JL; ++jl) {
+        const int j = 8 * jl + (lane >> 2);
+        if (j < R / 4) {
+          const int c = p.n0 + 8 * j + c_lane;
+          my_stats[c] += st[jl][0];
+          my_stats[c + 1] += st[jl][1];
+          my_stats[p.Cout + c] += st[jl][2];
+          my_stats[p.Cout + c + 1] += st[jl][3];
+        }
+      }
+      if (tile + (int)gridDim.x < p.num_tiles)
+        named_bar_arrive(kStatBar + (PIPE ? kNumEpiWarps : 0) + warp, 64);
     }
   };
 
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += 2 * gridDim.x) {
-    tile_fn(tile, 0, sa0, pa0, sb0, pb0);
-    if (tile + (int)gridDim.x < p.num_tiles) tile_fn(tile + gridDim.x, 1, sa1, pa1, sb1, pb1);
-  }
+  for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += tile_step) tile_fn(tile);
   if (p.stats) {   // this CTA's partial = the four warps' sums in warp order, then ordered over CTAs
-    auto bar = [] { asm volatile("bar.sync 1, %0;" ::"n"(kNumEpiWarps * 32) : "memory"); };
+    constexpr int kNt = kNumConsWarps * 32;
+    auto bar = [] { asm volatile("bar.sync 1, %0;" ::"n"(kNt) : "memory"); };
     bar();
     const int t = threadIdx.x, n = 2 * p.nn;
     double* slot = ordered_slot(p.red, 0, gridDim.x, blockIdx.x, n);
-    for (int i = t; i < n; i += kNumEpiWarps * 32) {
+    for (int i = t; i < n; i += kNt) {
       const int c = i < p.nn ? p.n0 + i : p.Cout + p.n0 + (i - p.nn);
       double v = 0.0;
       for (int w = 0; w < kNumEpiWarps; ++w) v += (double)s_stats[w * 2 * p.Cout + c];
       slot[i] = v;
     }
-    ordered_finish(p.red, 0, gridDim.x, n, t, kNumEpiWarps * 32, gridDim.x, bar,
+    ordered_finish(p.red, 0, gridDim.x, n, t, kNt, gridDim.x, bar,
                    [&](int i, double v) {
                      p.stats[i < p.nn ? p.n0 + i : p.Cout + p.n0 + (i - p.nn)] += v;
                    },
@@ -329,7 +417,8 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm,
 
 template <int U>
 __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ctl,
-                                            uint32_t a_base, uint32_t raw_base, int grp) {
+                                            uint32_t a_base, uint32_t raw_base, int grp,
+                                            const CUtensorMap* tm0, const CUtensorMap* tm1) {
   const int lane = threadIdx.x & 31;
   const int gt = threadIdx.x - (kFirstLoadWarp + grp * 4) * 32;   // 0..127
   const int P = p.KC >> 2;                   // planes per chunk (2, 4 or 8)
@@ -376,6 +465,32 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
   const uint32_t raw_src0 = raw_base + q0 * rowb + j * 16;
   const uint32_t bar_raw_full = smem_u32(&ctl->raw_full[0]), bar_raw_empty = smem_u32(&ctl->raw_empty[0]);
   uint32_t rst = 0, rph = 0;
+  // TMA mode: thread 0 of the group copies the raw tile of its k-chunk (r_tile, r_ch) into raw
+  // stage rs: one cp.async.bulk.tensor, box {KC channels, TWp, THp} at (c, w_org, h_org, n);
+  // coordinates outside the image are zero-filled by the copy engine
+  auto issue_raw = [&](int r_tile, int r_ch, uint32_t rs) {
+    const int n = r_tile / tpi, rem = r_tile - n * tpi;
+    const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
+    const int h_org = th_i * kTileH - p.dil * (p.taps_h >> 1);
+    const int w_org = tw_i * kTileW * p.sub - p.dil * (p.taps_w >> 1);
+    const uint32_t bar = bar_raw_full + (rr0 + rs) * 8;
+    mbar_arrive_expect_tx(bar, p.raw_bytes);
+    const int c = r_ch * p.KC, c_split = p.S.nsrc > 1 ? p.S.s[0].C : (1 << 30);
+    tma_load_4d(raw_base + (rr0 + rs) * p.raw_bytes, c < c_split ? tm0 : tm1,
+                c < c_split ? c : c - c_split, w_org, h_org, n, bar);
+  };
+  // the group's k-chunk `ahead` chunks after (r_tile, r_ch), or r_tile >= num_tiles past its last
+  auto chunk_after = [&](int& r_tile, int& r_ch, int ahead) {
+    r_ch += ahead;
+    while (r_ch >= n_chunks) { r_ch -= n_chunks; r_tile += tile_step; }
+  };
+  if (p.tma && gt == 0) {   // the first rn chunks; after that, one per transformed chunk
+    for (uint32_t i = 0; i < rn; ++i) {
+      int r_tile = tile, r_ch = 0;
+      chunk_after(r_tile, r_ch, (int)i);
+      if (r_tile < p.num_tiles) issue_raw(r_tile, r_ch, i);
+    }
+  }
   int ch = dual ? 0 : grp;
   uint32_t st = dual ? 0u : grp % n_a;
   uint32_t ph = dual ? 1u : ((grp / n_a) & 1) ^ 1;   // stage / empty-phase of the current chunk
@@ -547,6 +662,14 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
     if (lane == 0) mbar_arrive(bar_full_a + (ring0 + st) * 8);
     if (p.tma) {   // the raw tile has been consumed (the stores above depend on every load of it)
       if (lane == 0) mbar_arrive(bar_raw_empty + (rr0 + rst) * 8);
+      if (gt == 0) {   // once all four warps have read it, the stage takes the chunk rn later
+        int r_tile = tile, r_ch = ch;
+        chunk_after(r_tile, r_ch, (int)rn);
+        if (r_tile < p.num_tiles) {
+          mbar_wait_quiet(bar_raw_empty + (rr0 + rst) * 8, rph);
+          issue_raw(r_tile, r_ch, rst);
+        }
+      }
       if (++rst == rn) { rst = 0; rph ^= 1; }
     }
     // advance to this group's next chunk
@@ -554,6 +677,27 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
     st += ch_step;
     while (st >= ring_n) { st -= ring_n; ph ^= 1; }
   }
+}
+
+// consumer warpgroup PIPE: the instantiation for this launch's output channels and sub-tiles
+template <int PIPE>
+__device__ __forceinline__ void conv_consumer(const ConvTcParams& p, SharedCtl* ctl, uint32_t a_base,
+                                              uint32_t b_base, float* s_stats, const float* s_bias) {
+#define AB_CONS_CASE(NN, S) \
+  case NN: consumer_loop<NN, S, PIPE>(p, ctl, a_base, b_base, s_stats, s_bias); break;
+  if (p.sub == 2) {
+    switch (p.nn) {
+      AB_CONS_CASE(16, 2) AB_CONS_CASE(32, 2) AB_CONS_CASE(48, 2) AB_CONS_CASE(64, 2)
+      default: __trap();
+    }
+  } else {
+    switch (p.nn) {
+      AB_CONS_CASE(16, 1) AB_CONS_CASE(32, 1) AB_CONS_CASE(48, 1) AB_CONS_CASE(64, 1)
+      AB_CONS_CASE(80, 1) AB_CONS_CASE(96, 1) AB_CONS_CASE(112, 1) AB_CONS_CASE(128, 1)
+      default: __trap();
+    }
+  }
+#undef AB_CONS_CASE
 }
 
 constexpr int kCtlBytes = 1024;     // SharedCtl, then the statistics / bias block
@@ -573,17 +717,13 @@ __global__ void __launch_bounds__(kThreads, 1)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int taps = p.taps_h * p.taps_w;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.n_a; ++i) {
       mbar_init(smem_u32(&ctl->full_a[i]), kNumLoadWarps / 2);
       mbar_init(smem_u32(&ctl->empty_a[i]), kNumEpiWarps);
     }
-    for (int i = 0; i < p.n_b; ++i) {
-      mbar_init(smem_u32(&ctl->full_b[i]), 1);
-      mbar_init(smem_u32(&ctl->empty_b[i]), kNumEpiWarps);
-    }
+    for (int i = 0; i < p.n_b; ++i) mbar_init(smem_u32(&ctl->full_b[i]), 1);
     for (int i = 0; i < kMaxRStages; ++i) {
       mbar_init(smem_u32(&ctl->raw_full[i]), 1);
       mbar_init(smem_u32(&ctl->raw_empty[i]), kNumLoadWarps / 2);
@@ -598,7 +738,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   }
   __syncthreads();
 
-  if (warp >= kFirstLoadWarp && warp < kEpiBWarp) {
+  if (warp >= kFirstLoadWarp) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsLoad));
     // ===================== activation loaders =====================
     // Two groups of 4 warps; group g stages every k-chunk of the tiles with local index = g
@@ -609,102 +749,33 @@ __global__ void __launch_bounds__(kThreads, 1)
     const int grp = (warp - kFirstLoadWarp) >> 2;
     const int U = (p.HP * (p.KC >> 2) + kGroupThreads - 1) / kGroupThreads;   // <= kMaxU (plan)
     switch (U) {
-#define AB_LOAD_CASE(K) case K: loader_loop<K>(p, ctl, a_base, raw_base, grp); break;
+#define AB_LOAD_CASE(K) case K: loader_loop<K>(p, ctl, a_base, raw_base, grp, &tm0, &tm1); break;
       AB_LOAD_CASE(1) AB_LOAD_CASE(2) AB_LOAD_CASE(3) AB_LOAD_CASE(4) AB_LOAD_CASE(5) AB_LOAD_CASE(6)
       AB_LOAD_CASE(7) AB_LOAD_CASE(8) AB_LOAD_CASE(9) AB_LOAD_CASE(10) AB_LOAD_CASE(11)
       AB_LOAD_CASE(12)
 #undef AB_LOAD_CASE
       default: __trap();
     }
-  } else if (warp >= kNumEpiWarps && warp < kFirstLoadWarp) {
-   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsMma));
-   if (warp == kWgtWarp || (warp == kWgtWarp2 && (!p.w_resident || p.tma))) {
-    // ===================== weight producer(s) / TMA activation producers =====================
-    if (elect_one()) {
-      if (p.w_resident) {
-        if (warp == kWgtWarp) {
-          // the packed blob is already in shared-memory order: copy it once, in 16 KB pieces
-          const uint32_t bar = smem_u32(&ctl->w_full);
-          mbar_arrive_expect_tx(bar, p.w_bytes);
-          for (int off = 0; off < p.w_bytes; off += 16384) {
-            const int n = min(16384, p.w_bytes - off);
-            bulk_g2s(b_base + off, reinterpret_cast<const char*>(p.wblob) + off, n, bar);
-          }
-        }
-        if (p.tma) {
-          // warp 5 feeds pipeline 0's raw ring, warp 7 pipeline 1's: one cp.async.bulk.tensor per
-          // (tile, k-chunk): box {KC channels, TWp, THp} at (c, w_org, h_org, n); coordinates
-          // outside the image are zero-filled by the copy engine
-          const int pipe = warp == kWgtWarp ? 0 : 1;
-          const uint32_t rn = (uint32_t)p.n_r / 2, rr0 = pipe * rn;
-          const uint32_t bar_full = smem_u32(&ctl->raw_full[0]), bar_empty = smem_u32(&ctl->raw_empty[0]);
-          const int tpi = p.tiles_w * p.tiles_h;
-          const int c_split = p.S.nsrc > 1 ? p.S.s[0].C : (1 << 30);
-          uint32_t rs = 0, rph = 1;
-          for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += 2 * gridDim.x) {
-            const int n = tile / tpi, rem = tile - n * tpi;
-            const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
-            const int h_org = th_i * kTileH - p.dil * (p.taps_h >> 1);
-            const int w_org = tw_i * kTileW * p.sub - p.dil * (p.taps_w >> 1);
-            for (int ch = 0; ch < p.n_chunks; ++ch) {
-              mbar_wait_quiet(bar_empty + (rr0 + rs) * 8, rph);
-              const uint32_t bar = bar_full + (rr0 + rs) * 8;
-              mbar_arrive_expect_tx(bar, p.raw_bytes);
-              const int c = ch * p.KC;
-              tma_load_4d(raw_base + (rr0 + rs) * p.raw_bytes, c < c_split ? &tm0 : &tm1,
-                          c < c_split ? c : c - c_split, w_org, h_org, n, bar);
-              if (++rs == rn) { rs = 0; rph ^= 1; }
-            }
-          }
-        }
-      } else {
-        // streamed: producer i (warp 5 / warp 7) feeds pipeline i's weight ring for its tiles
-        const int pipe = warp == kWgtWarp ? 0 : 1;
-        const uint32_t nb2 = p.n_b / 2, ring0 = pipe * nb2;
-        uint32_t st = 0, ph = 1;
-        const int ksteps = p.KC >> 3;
-        const uint32_t piece = p.Cout * 32;  // bytes of one (k-step, tap) piece
-        const uint32_t b_stage = p.b_stage_bytes;
-        const uint32_t bar_full_b = smem_u32(&ctl->full_b[0]), bar_empty_b = smem_u32(&ctl->empty_b[0]);
-        for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += 2 * gridDim.x) {
-          const int wmult = p.x3 ? 2 : 1;
-          for (int ch = 0; ch < p.n_chunks; ++ch) {
-            for (int t = 0; t < taps; ++t) {
-              mbar_wait_quiet(bar_empty_b + (ring0 + st) * 8, ph);
-              const uint32_t bar = bar_full_b + (ring0 + st) * 8;
-              mbar_arrive_expect_tx(bar, b_stage);
-              // piece (k-step s, kind, tap) of the blob lives at ((s*wmult + kind)*taps + tap);
-              // the stage holds [k-step][kind] pieces
-              for (int ks = 0; ks < ksteps; ++ks)
-                for (int kd = 0; kd < wmult; ++kd)
-                  bulk_g2s(b_base + (ring0 + st) * b_stage + (ks * wmult + kd) * piece,
-                           p.wblob + ((((size_t)ch * ksteps + ks) * wmult + kd) * taps + t) * (piece >> 2),
-                           piece, bar);
-              if (++st == nb2) { st = 0; ph ^= 1; }
-            }
-          }
-        }
-      }
-    }
-    __syncwarp();
-   }
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsEpi));
-    // ===================== consumer: wgmma + epilogue =====================
-#define AB_CONS_CASE(NN, S) case NN: consumer_loop<NN, S>(p, ctl, a_base, b_base, s_stats, s_bias); break;
-    if (p.sub == 2) {
-      switch (p.nn) {
-        AB_CONS_CASE(16, 2) AB_CONS_CASE(32, 2) AB_CONS_CASE(48, 2) AB_CONS_CASE(64, 2)
-        default: __trap();
-      }
-    } else {
-      switch (p.nn) {
-        AB_CONS_CASE(16, 1) AB_CONS_CASE(32, 1) AB_CONS_CASE(48, 1) AB_CONS_CASE(64, 1)
-        AB_CONS_CASE(80, 1) AB_CONS_CASE(96, 1) AB_CONS_CASE(112, 1) AB_CONS_CASE(128, 1)
-        default: __trap();
+    // ===================== consumers: wgmma + epilogue =====================
+    if (p.w_resident && threadIdx.x == 0) {
+      // the packed blob is already in shared-memory order: copy it once, in 16 KB pieces
+      const uint32_t bar = smem_u32(&ctl->w_full);
+      mbar_arrive_expect_tx(bar, p.w_bytes);
+      for (int off = 0; off < p.w_bytes; off += 16384) {
+        const int n = min(16384, p.w_bytes - off);
+        bulk_g2s(b_base + off, reinterpret_cast<const char*>(p.wblob) + off, n, bar);
       }
     }
-#undef AB_CONS_CASE
+    // one branch per consumer ahead of setmaxnreg (.sync.aligned: each warpgroup is converged
+    // after it), so nothing in a consumer's wgmma code depends on the thread index
+    if (warp < kNumEpiWarps) {
+      asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsCons));
+      conv_consumer<0>(p, ctl, a_base, b_base, s_stats, s_bias);
+    } else {
+      asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsCons));
+      conv_consumer<1>(p, ctl, a_base, b_base, s_stats, s_bias);
+    }
   }
   __syncthreads();
 }
