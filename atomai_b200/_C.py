@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "libatomai_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
-           "segloss.cu", "refine.cu"]
+           "segloss.cu", "refine.cu", "jlatent.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -28,6 +28,10 @@ MATH_TF32X3 = 2
 WMODE_FWD = 0
 WMODE_DGRAD = 1
 REFINE_NONFINITE = -2    # AB_REFINE_NONFINITE of include/atomai_b200.h
+JLAT_MAX_CONT = 32       # AB_JLAT_MAX_CONT
+JLAT_MAX_DISC = 64       # AB_JLAT_MAX_DISC
+JLAT_ALPHAS = 0
+JLAT_SAMPLE = 1
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -65,6 +69,12 @@ class CoordLat(C.Structure):
                 ("hid", C.c_int32), ("tanh_act", C.c_int32),
                 ("z", C.c_void_p), ("phi", C.c_void_p), ("dx", C.c_void_p),
                 ("wc", C.c_void_p), ("bc", C.c_void_p), ("wz", C.c_void_p)]
+
+
+class JLat(C.Structure):
+    _fields_ = [("B", C.c_int32), ("Dc", C.c_int32), ("coord", C.c_int32), ("nheads", C.c_int32),
+                ("heads", C.c_int32 * JLAT_MAX_DISC), ("tau", C.c_float), ("phi_prior", C.c_float),
+                ("dx_prior", C.c_float)]
 
 
 _vp, _i, _i64, _f, _d = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
@@ -117,6 +127,10 @@ SIGNATURES = {
     "atomai_b200_coord_latent_fwd": (_i, [C.POINTER(CoordLat), _vp, _vp]),
     "atomai_b200_coord_latent_bwd": (_i, [C.POINTER(CoordLat), _vp, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
+    "atomai_b200_jlatent_fwd": (_i, [C.POINTER(JLat), _i, _vp, _vp, _vp, _vp, _vp, C.c_uint64, _vp,
+                                     _vp, _vp, _vp, _vp, _vp]),
+    "atomai_b200_jlatent_bwd": (_i, [C.POINTER(JLat), _i, _vp, _vp, _vp, _vp, _vp, C.c_uint64, _vp,
+                                     _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "atomai_b200_sqerr_reduce": (_i, [_vp, _vp, _i64, _vp, _vp, _f, _vp, _vp]),
     "atomai_b200_gram_workspace_bytes": (_i64, [_i, _i, _i]),
     "atomai_b200_gram": (_i, [_vp, _vp, _vp, _f, _i, _i, _i, _i, _i, _vp, _i64, _vp, _i64, _vp]),

@@ -70,6 +70,16 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   return v;
 }
 
+// Counter-based RNG shared by dropout and the Gumbel noise of the joint VAEs: a 64-bit mix of the
+// counter and the seed (splitmix64 finaliser), top 24 bits -> uniform in [0, 1)
+__device__ __forceinline__ float hash_uniform(uint64_t idx, uint64_t seed) {
+  uint64_t z = idx + seed * 0x9E3779B97F4A7C15ull + 0xD1B54A32D192ED03ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z ^= z >> 31;
+  return (float)(uint32_t)(z >> 40) * (1.0f / 16777216.0f);
+}
+
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));

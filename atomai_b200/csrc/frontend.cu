@@ -62,15 +62,6 @@ __global__ void __launch_bounds__(kT) gather_windows_kernel(const float* __restr
   if (nanflag && __syncthreads_or(bad) && threadIdx.x == 0) nanflag[k] = 1;
 }
 
-// 32-bit mix (lowbias32-style finaliser) of a 64-bit counter and the seed: uniform in [0, 1)
-__device__ __forceinline__ float hash_uniform(uint64_t idx, uint64_t seed) {
-  uint64_t z = idx + seed * 0x9E3779B97F4A7C15ull + 0xD1B54A32D192ED03ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  z ^= z >> 31;
-  return (float)(uint32_t)(z >> 40) * (1.0f / 16777216.0f);
-}
-
 __global__ void __launch_bounds__(kT) dropout_kernel(float* __restrict__ a, int ld, int64_t npix,
                                                       int C, float p, float inv_keep, uint64_t seed,
                                                       double* __restrict__ stats) {

@@ -1,7 +1,7 @@
-from .dgm import VAE, BaseVAE, rVAE
+from .dgm import VAE, BaseVAE, jrVAE, jVAE, rVAE
 from .dklgp import dklGPR
 from .imspec import ImSpec
 from .loaders import load_model
 from .segmentor import Segmentor
 
-__all__ = ["Segmentor", "ImSpec", "VAE", "rVAE", "BaseVAE", "dklGPR", "load_model"]
+__all__ = ["Segmentor", "ImSpec", "VAE", "rVAE", "jVAE", "jrVAE", "BaseVAE", "dklGPR", "load_model"]

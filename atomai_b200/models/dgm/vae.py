@@ -21,8 +21,9 @@ class BaseVAE(viBaseTrainer):
     General class for VAE models (atomai/models/dgm/vae.py:28-103).
 
     Args: in_dim, latent_dim, nb_classes, coord (0: VAE, 1: rotation, 2: translation,
-    3: rotation + translation), discrete_dim (unsupported), seed, and the **kwargs of
-    init_VAE_nets (conv_encoder, conv_decoder, numlayers_*, numhidden_*, ...).
+    3: rotation + translation), discrete_dim (sizes of the Gumbel-softmax latents of jVAE /
+    jrVAE), seed, and the **kwargs of init_VAE_nets (conv_encoder, conv_decoder, numlayers_*,
+    numhidden_*, ...).
     """
     def __init__(self, in_dim: Tuple[int], latent_dim: int, nb_classes: int = 0, coord: int = 0,
                  discrete_dim: Optional[List] = None, seed: int = 0,
@@ -39,6 +40,8 @@ class BaseVAE(viBaseTrainer):
         np.random.seed(seed)
         self.in_dim = in_dim
         self.z_dim = latent_dim
+        if discrete_dim:
+            self.z_dim = self.z_dim + sum(discrete_dim)
         self.discrete_dim = discrete_dim
         if coord:
             if len(in_dim) not in (2, 3):
@@ -59,8 +62,8 @@ class BaseVAE(viBaseTrainer):
     # ------------------------------------------------------------------ inference API
     def encode_(self, x_new: Union[np.ndarray, torch.Tensor], **kwargs: int
                 ) -> Tuple[np.ndarray]:
-        """Encodes input data batch-by-batch; returns (z_mean, z_sd) numpy arrays
-        (vae.py:105-147)."""
+        """Encodes input data batch-by-batch; returns (z_mean, z_sd) numpy arrays, and for the
+        joint VAEs also the (N, sum(discrete_dim)) alphas (vae.py:105-176)."""
         if isinstance(x_new, np.ndarray):
             x_new = torch.from_numpy(x_new).float()
         if (x_new.ndim == len(self.in_dim) == 2 or x_new.ndim == len(self.in_dim) == 3):
@@ -68,12 +71,16 @@ class BaseVAE(viBaseTrainer):
         num_batches = kwargs.get("num_batches", 10)
         batch_size = max(len(x_new) // num_batches, 1)
         self.encoder_net.eval()
-        mus, sds = [], []
+        mus, sds, alphas = [], [], []
         with torch.no_grad():
             for i in range(0, len(x_new), batch_size):
-                z_mean, z_logsd = self.encoder_net(x_new[i:i + batch_size].to(self.device))
+                z_mean, z_logsd, *alpha = self.encoder_net(x_new[i:i + batch_size].to(self.device))
                 mus.append(z_mean.cpu())
                 sds.append(torch.exp(z_logsd).cpu())
+                if alpha:
+                    alphas.append(torch.cat(alpha, 1).cpu())
+        if alphas:
+            return torch.cat(mus).numpy(), torch.cat(sds).numpy(), torch.cat(alphas).numpy()
         return torch.cat(mus).numpy(), torch.cat(sds).numpy()
 
     def encode(self, x_new, **kwargs: int) -> Tuple[np.ndarray]:
@@ -85,6 +92,9 @@ class BaseVAE(viBaseTrainer):
         coordinate on the CPU; here the image lives on the GPU, every batch of windows is one
         gather kernel and goes straight into the encoder.  Returns the cropped original image
         and the (h', w', z_dim) encoded array (cropping is due to the finite window size)."""
+        if self.discrete_dim:
+            raise NotImplementedError("encode_image_ of the joint VAEs (the reference's cannot "
+                                      "unpack their three outputs either)")
         from ...utils.img import crop_borders, extract_subimages_cuda, get_coord_grid
         num_batches = kwargs.get("num_batches", 10)
         inf = int(1e5)
@@ -142,11 +152,24 @@ class BaseVAE(viBaseTrainer):
         return x_decoded.cpu().numpy()
 
     def reconstruct(self, x_new, **kwargs: int) -> np.ndarray:
-        """encode -> decode of the latent mean (vae.py:223-247)."""
-        z_mean, _ = self.encode(x_new, **kwargs)
-        if self.coord > 0:
-            z_mean = z_mean[:, self.coord:]
-        return self.decode(z_mean)
+        """encode -> decode of the latent mean (vae.py:223-271).  The joint VAEs append the encoded
+        alphas, or with `label` (an int, or one int per discrete head) the one-hot class vector."""
+        if not self.discrete_dim:
+            z_mean, _ = self.encode(x_new, **kwargs)
+            if self.coord > 0:
+                z_mean = z_mean[:, self.coord:]
+            return self.decode(z_mean)
+        z_mean, _, alphas = self.encode(x_new, **kwargs)
+        z_mean = z_mean[:, self.coord:]
+        label = kwargs.get("label")
+        if label is not None:
+            labels = [label] if np.ndim(label) == 0 else list(label)
+            if len(labels) != len(self.discrete_dim):
+                raise ValueError("pass one label per discrete latent")
+            onehot = np.concatenate([np.eye(d, dtype=np.float32)[int(k)]
+                                     for k, d in zip(labels, self.discrete_dim)])
+            alphas = np.broadcast_to(onehot, (len(z_mean), len(onehot)))
+        return self.decode(np.concatenate([z_mean, alphas], 1).astype(np.float32))
 
     # ------------------------------------------------------------------ training helpers
     def _check_inputs(self, X_train, y_train=None, X_test=None, y_test=None) -> None:
@@ -159,14 +182,15 @@ class BaseVAE(viBaseTrainer):
         self.metadict["num_epochs"] = self.current_epoch
         self.metadict["num_iter"] = self.kdict_["num_iter"]
 
-    def _fit_loop(self, **kwargs) -> None:
+    def _fit_loop(self, _print_stats: bool = True, **kwargs) -> None:
         for e in range(self.training_cycles):
             self.current_epoch = e
             elbo_epoch = self.train_epoch()
             self.loss_history["train_loss"].append(elbo_epoch)
             if self.test_iterator is not None:
                 self.loss_history["test_loss"].append(self.evaluate_model())
-            self.print_statistics(e)
+            if _print_stats:
+                self.print_statistics(e)
             self.update_metadict()
             if kwargs.get("save_every_epoch", True):
                 self.save_model(self.filename)

@@ -57,7 +57,7 @@ def load_imspec_model(meta_dict):
 
 
 def load_vae_model(meta_dict):
-    from .dgm import VAE, rVAE
+    from .dgm import VAE, jrVAE, jVAE, rVAE
     meta = dict(meta_dict)
     meta.pop("model_type", None)
     coord = meta.get("coord", 0)
@@ -65,12 +65,16 @@ def load_vae_model(meta_dict):
     optimizer = meta.pop("optimizer", None)
     in_dim, latent_dim = meta.pop("in_dim"), meta.pop("latent_dim")
     meta.pop("coord", None)
-    # any non-zero coord is an rVAE; coord == 3 adds translation (atomai/models/loaders.py:163-195)
+    # any non-zero coord is an rVAE; coord == 3 adds translation; a non-empty discrete_dim makes
+    # the joint models (atomai/models/loaders.py:163-195)
+    joint = bool(meta.get("discrete_dim"))
     if coord:
         meta.pop("translation", None)
-        m = rVAE(in_dim, latent_dim, translation=(coord == 3), **meta)
+        m = (jrVAE if joint else rVAE)(in_dim, latent_dim, translation=(coord == 3), **meta)
     else:
-        m = VAE(in_dim, latent_dim, **meta)
+        m = (jVAE if joint else VAE)(in_dim, latent_dim, **meta)
+    if joint:
+        m.kdict_["num_iter"] = meta.get("num_iter", 0)
     m.encoder_net.load_state_dict(enc)
     m.encoder_net.eval()
     m.decoder_net.load_state_dict(dec)

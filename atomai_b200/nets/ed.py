@@ -7,8 +7,8 @@ Each network is one autograd node per call; inside it the ConvBlocks run on the 
 convolution kernels, `x.reshape(-1, C*H*W) -> nn.Linear` becomes an NHWC->NCHW transpose kernel +
 a split-K GEMM, and the rVAE spatial decoder (coord_latent + transform_coordinates + per-pixel MLP)
 is a fused coordinate kernel followed by 1x1 tensor-core convolutions with tanh epilogues.
-
-jfcEncoderNet / jconvEncoderNet (joint VAEs) are out of the hot-path scope (SURVEY.md §2.1).
+The joint encoders (jfcEncoderNet / jconvEncoderNet, atomai/nets/ed.py:346-468) add one skinny
+Linear per discrete head; their softmax is the joint-latent kernel (losses_metrics/vi_losses.py).
 """
 from typing import Dict, List, Optional, Tuple, Type, Union
 
@@ -18,6 +18,7 @@ import torch.nn as nn
 
 from .. import engine
 from ..engine import ACT_LRELU, ACT_TANH, Act, Tape
+from ..losses_metrics.vi_losses import joint_alphas
 from .blocks import ConvBlock, DilatedBlock
 
 
@@ -173,16 +174,20 @@ class convEncoderNet(nn.Module):
         return tape.linear(flat, self.fc11), tape.linear(flat, self.fc12)
 
     def forward(self, x: torch.Tensor) -> Tuple[torch.Tensor]:
-        if x.ndim == 2:                      # (B, L) spectra -> (B,1,L,1)
-            xin = x.reshape(x.shape[0], 1, x.shape[1], 1)
-        elif x.ndim == 3:                    # (B, H, W) -> NHWC with C = 1
-            xin = x.unsqueeze(-1)
-        else:                                # (B, H, W, C) is already channel-last
-            xin = x
-        xin = xin.float().contiguous()
-        z_mu, z_ls = engine.run_multi(self, self._emit, (xin,))
+        z_mu, z_ls = engine.run_multi(self, self._emit, (_conv_enc_input(x),))
         z_mu, z_ls = z_mu.reshape(z_mu.shape[0], -1), z_ls.reshape(z_ls.shape[0], -1)
         return z_mu, self._out(z_ls)
+
+
+def _conv_enc_input(x: torch.Tensor) -> torch.Tensor:
+    """Input of the convolutional encoders as a contiguous NHWC batch."""
+    if x.ndim == 2:                      # (B, L) spectra -> (B,1,L,1)
+        xin = x.reshape(x.shape[0], 1, x.shape[1], 1)
+    elif x.ndim == 3:                    # (B, H, W) -> NHWC with C = 1
+        xin = x.unsqueeze(-1)
+    else:                                # (B, H, W, C) is already channel-last
+        xin = x
+    return xin.float().contiguous()
 
 
 class fcEncoderNet(nn.Module):
@@ -214,6 +219,67 @@ class fcEncoderNet(nn.Module):
         z_mu, z_ls = engine.run_multi(self, self._emit, (xin,))
         z_mu, z_ls = z_mu.reshape(z_mu.shape[0], -1), z_ls.reshape(z_ls.shape[0], -1)
         return z_mu, self._out(z_ls)
+
+
+def _joint_heads(net: nn.Module, xin: torch.Tensor):
+    """(z_mean, z_logsd after the optional softplus, the discrete heads' logits concatenated) of a
+    joint encoder: trunk, fc11, fc12 and one skinny Linear per head in one native graph."""
+    z_mu, z_ls, *logits = engine.run_multi(net, net._emit, (xin,))
+    b = z_mu.shape[0]
+    return (z_mu.reshape(b, -1), net._out(z_ls.reshape(b, -1)),
+            torch.cat([lg.reshape(b, -1) for lg in logits], 1))
+
+
+class jfcEncoderNet(fcEncoderNet):
+    """
+    MLP encoder for joint continuous and discrete latents (atomai/nets/ed.py:346-407):
+    num_layers x (Linear + tanh) -> fc11 / fc12 / fc13[i] (one Linear per discrete head).
+    forward(x) returns [z_mean, z_logsd, alpha_1, ..., alpha_n] as the reference does.
+    """
+    def __init__(self, in_dim: Tuple[int], latent_dim: int = 2, discrete_dim: List = [1],
+                 num_layers: int = 2, hidden_dim: int = 32, **kwargs: bool) -> None:
+        super(jfcEncoderNet, self).__init__(in_dim, latent_dim, num_layers, hidden_dim, **kwargs)
+        self.fc13 = nn.ModuleList([nn.Linear(self.reshape_, d) for d in discrete_dim])
+        self.discrete_dim = [int(d) for d in discrete_dim]
+
+    def _emit(self, tape: Tape, x: Act):
+        for m in self.dense:
+            if isinstance(m, nn.Linear):
+                x = tape.linear(x, m, ACT_TANH)
+        return tuple(tape.linear(x, m) for m in (self.fc11, self.fc12, *self.fc13))
+
+    def heads(self, x: torch.Tensor):
+        """(z_mean, z_logsd, concatenated head logits): what the joint training step consumes."""
+        return _joint_heads(self, _vec(x.reshape(x.shape[0], -1).float().contiguous()))
+
+    def forward(self, x: torch.Tensor) -> List[torch.Tensor]:
+        z_mu, z_ls, logits = self.heads(x)
+        return [z_mu, z_ls, *torch.split(joint_alphas(logits, self.discrete_dim), self.discrete_dim, 1)]
+
+
+class jconvEncoderNet(convEncoderNet):
+    """
+    Convolutional encoder for joint continuous and discrete latents (atomai/nets/ed.py:410-468):
+    ConvBlock(num_layers, c -> hidden_dim, lrelu 0.1) -> flatten -> fc11 / fc12 / fc13[i].
+    forward(x) returns [z_mean, z_logsd, alpha_1, ..., alpha_n] as the reference does.
+    """
+    def __init__(self, in_dim: Tuple[int], latent_dim: int = 2, discrete_dim: List = [1],
+                 num_layers: int = 2, hidden_dim: int = 32, **kwargs: Union[float, bool]) -> None:
+        super(jconvEncoderNet, self).__init__(in_dim, latent_dim, num_layers, hidden_dim, **kwargs)
+        self.fc13 = nn.ModuleList([nn.Linear(self.reshape_, d) for d in discrete_dim])
+        self.discrete_dim = [int(d) for d in discrete_dim]
+
+    def _emit(self, tape: Tape, x: Act):
+        flat = tape.flatten(self.conv._emit(tape, x))
+        return tuple(tape.linear(flat, m) for m in (self.fc11, self.fc12, *self.fc13))
+
+    def heads(self, x: torch.Tensor):
+        """(z_mean, z_logsd, concatenated head logits): what the joint training step consumes."""
+        return _joint_heads(self, _conv_enc_input(x))
+
+    def forward(self, x: torch.Tensor) -> List[torch.Tensor]:
+        z_mu, z_ls, logits = self.heads(x)
+        return [z_mu, z_ls, *torch.split(joint_alphas(logits, self.discrete_dim), self.discrete_dim, 1)]
 
 
 class convDecoderNet(nn.Module):
@@ -399,9 +465,9 @@ def init_imspec_model(in_dim: Tuple[int], out_dim: Tuple[int], latent_dim: int,
 def init_VAE_nets(in_dim: Tuple[int], latent_dim: int, coord: int = 0,
                   discrete_dim: Optional[List] = None, nb_classes: int = 0, **kwargs
                   ) -> Tuple[Type[nn.Module], Type[nn.Module], Dict[str, Union[int, bool]]]:
-    """Initializes encoder and decoder for VAE + meta dict (atomai/nets/ed.py:725-790)."""
-    if discrete_dim:
-        raise NotImplementedError("joint (discrete) VAEs are outside the atomai_b200 hot path")
+    """Initializes encoder and decoder for VAE + meta dict (atomai/nets/ed.py:725-790).  With
+    `discrete_dim` the encoder gets one head per discrete latent and the decoder takes
+    latent_dim + sum(discrete_dim) inputs (class conditioning is then off)."""
     conv_e = kwargs.get("conv_encoder", False)
     conv_d = kwargs.get("conv_decoder", False) if not coord else None
     numlayers_e = kwargs.get("numlayers_encoder", 2)
@@ -411,14 +477,22 @@ def init_VAE_nets(in_dim: Tuple[int], latent_dim: int, coord: int = 0,
     skip = kwargs.get("skip", False)
     sigmoid_out = kwargs.get("sigmoid_out", False)
     softplus_out = kwargs.get("softplus_out")
+    discrete_dim_ = sum(discrete_dim) if discrete_dim else 0
+    nb_classes_ = nb_classes if discrete_dim_ == 0 else 0
     if not coord:
         dnet = convDecoderNet if conv_d else fcDecoderNet
-        decoder_net = dnet(in_dim, latent_dim + nb_classes, numlayers_d, numhidden_d)
+        decoder_net = dnet(in_dim, latent_dim + discrete_dim_ + nb_classes_, numlayers_d, numhidden_d)
     else:
-        decoder_net = rDecoderNet(in_dim, latent_dim + nb_classes, numlayers_d, numhidden_d, skip)
-    enet = convEncoderNet if conv_e else fcEncoderNet
-    encoder_net = enet(in_dim, latent_dim + coord, numlayers_e, numhidden_e,
-                       softplus_out=softplus_out)
+        decoder_net = rDecoderNet(in_dim, latent_dim + discrete_dim_ + nb_classes_, numlayers_d,
+                                  numhidden_d, skip)
+    if not discrete_dim:
+        enet = convEncoderNet if conv_e else fcEncoderNet
+        encoder_net = enet(in_dim, latent_dim + coord, numlayers_e, numhidden_e,
+                           softplus_out=softplus_out)
+    else:
+        enet = jconvEncoderNet if conv_e else jfcEncoderNet
+        encoder_net = enet(in_dim, latent_dim + coord, discrete_dim, numlayers_e, numhidden_e,
+                           softplus_out=softplus_out)
     meta_state_dict = {
         "model_type": "vae", "in_dim": in_dim, "latent_dim": latent_dim, "coord": coord,
         "conv_encoder": conv_e, "numlayers_encoder": numlayers_e,

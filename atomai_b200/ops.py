@@ -360,6 +360,46 @@ def coord_latent_bwd(d: _C.CoordLat, dpre0, dwc, dbc, sb, dphi, ddx) -> None:
                                              ptr(dphi), ptr(ddx), stream_ptr()))
 
 
+def jlat_desc(B, Dc, coord, heads, tau, phi_prior=0.1, dx_prior=0.1) -> _C.JLat:
+    """Descriptor of the joint latent block: B rows, Dc continuous columns (coord of them rotation /
+    translation), discrete heads of sizes `heads`, Gumbel-softmax temperature tau."""
+    if not 1 <= len(heads) <= _C.JLAT_MAX_DISC:
+        raise ValueError(f"joint latent: {len(heads)} discrete heads (1..{_C.JLAT_MAX_DISC})")
+    d = _C.JLat()
+    d.B, d.Dc, d.coord, d.nheads = int(B), int(Dc), int(coord), len(heads)
+    for i, h in enumerate(heads):
+        d.heads[i] = int(h)
+    d.tau, d.phi_prior, d.dx_prior = float(tau), float(phi_prior), float(dx_prior)
+    return d
+
+
+def _check_args(status: int) -> None:
+    """check() for entry points whose failures are arguments outside their documented limits."""
+    try:
+        check(status)
+    except _C.NativeError as e:
+        raise ValueError(str(e)) from None
+
+
+def jlatent_fwd(d: _C.JLat, mode: int, mu, logsd, logits, eps, u, seed: int, alpha, zdec=None,
+                phi=None, dx=None, kl=None) -> None:
+    """alpha (B, D) <- head softmax of logits; mode JLAT_SAMPLE also writes the decoder input zdec,
+    phi / dx (coord > 0) and kl = [continuous KL mean, discrete KL sum of means] (nullable).  The
+    Gumbel noise comes from `u` (B, D) when given, else from the hash generator with `seed`."""
+    _check_args(lib().atomai_b200_jlatent_fwd(
+        C.byref(d), mode, ptr(mu), ptr(logsd), ptr(logits), ptr(eps), ptr(u), int(seed) & (2**64 - 1),
+        ptr(alpha), ptr(zdec), ptr(phi), ptr(dx), ptr(kl), stream_ptr()))
+
+
+def jlatent_bwd(d: _C.JLat, mode: int, mu, logsd, logits, eps, u, seed: int, dzdec, dphi, ddx,
+                dalpha, gkl, dmu, dlogsd, dlogits) -> None:
+    """Gradients of jlatent_fwd w.r.t. mu, logsd and logits (every incoming gradient nullable)."""
+    _check_args(lib().atomai_b200_jlatent_bwd(
+        C.byref(d), mode, ptr(mu), ptr(logsd), ptr(logits), ptr(eps), ptr(u), int(seed) & (2**64 - 1),
+        ptr(dzdec), ptr(dphi), ptr(ddx), ptr(dalpha), ptr(gkl), ptr(dmu), ptr(dlogsd), ptr(dlogits),
+        stream_ptr()))
+
+
 def gram(x1, x2, inv_ls, outputscale, kind, out, math=MATH_TF32X3) -> None:
     n1, d = x1.shape
     n2 = x2.shape[0]

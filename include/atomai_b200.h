@@ -282,6 +282,44 @@ int atomai_b200_coord_latent_bwd(const ab_coordlat_t* d, const float* dpre0, flo
 int atomai_b200_sqerr_reduce(const float* x, const float* xhat, int64_t n, double* out,
                              float* dxhat, float gscale, const float* gscale_dev, void* stream);
 
+/* ---- joint (continuous + Gumbel-softmax) latent block of jVAE / jrVAE ------------------------
+ * (atomai/models/dgm/jvae.py:103-131, jrvae.py:117-151, trainers/vitrainer.py:236-248,
+ * losses_metrics/vi_losses.py:40-84,140-221).  Per row b of B, with D = sum of the head sizes:
+ *   alpha = softmax(logits) per head (fp32, max subtracted)
+ *   z     = mu + exp(logsd) * eps                                   (Dc continuous columns)
+ *   g     = -log(-log(u + 1e-12) + 1e-12),  u = caller's uniform or hash(seed, b*D + j)
+ *   zd    = softmax((log(alpha + 1e-12) + g) / tau) per head
+ *   zdec  = [z[coord:], zd]  (B x (Dc - coord + D): the decoder input),  phi = z[:, 0] and
+ *           dx = z[:, 1:3] * dx_prior when coord is 1 / 3 (rDecoderNet's rotation / translation)
+ *   kl[0] = mean_b kld_normal(z columns coord>0 ? 1.. : 0..) + (coord ? mean_b kld_rot(logsd[:,0]) : 0)
+ *   kl[1] = sum_heads mean_b sum_j alpha (log(alpha + 1e-12) - log(1/D_h + 1e-12))
+ * The KL sums run in fp64 in a fixed order in one CTA (no atomics): one input, one output bit
+ * pattern.  Limits: 1 <= Dc <= 32, coord in {0, 1, 3} < Dc, 1 <= D <= 64 (any number of heads).
+ * mode AB_JLAT_ALPHAS computes alpha only (mu, logsd, eps, u, zdec, phi, dx, kl unused). */
+#define AB_JLAT_MAX_CONT 32
+#define AB_JLAT_MAX_DISC 64
+#define AB_JLAT_ALPHAS 0
+#define AB_JLAT_SAMPLE 1
+typedef struct {
+  int32_t B, Dc, coord, nheads;
+  int32_t heads[AB_JLAT_MAX_DISC]; /* head sizes D_1..D_nheads */
+  float tau, phi_prior, dx_prior;
+} ab_jlat_t;
+/* u: [B][D] or NULL (then the hash generator with `seed`); phi, dx: [B], [B][2] when coord > 0;
+ * kl: float[2] or NULL */
+int atomai_b200_jlatent_fwd(const ab_jlat_t* d, int mode, const float* mu, const float* logsd,
+                            const float* logits, const float* eps, const float* u, uint64_t seed,
+                            float* alpha, float* zdec, float* phi, float* dx, float* kl,
+                            void* stream);
+/* Gradients of the forward above (same inputs, same noise) from dzdec, dphi, ddx, dalpha and
+ * gkl = d loss / d kl[0..1] (each nullable = zero); overwrites dmu, dlogsd ([B][Dc], unused in
+ * mode AB_JLAT_ALPHAS) and dlogits ([B][D]). */
+int atomai_b200_jlatent_bwd(const ab_jlat_t* d, int mode, const float* mu, const float* logsd,
+                            const float* logits, const float* eps, const float* u, uint64_t seed,
+                            const float* dzdec, const float* dphi, const float* ddx,
+                            const float* dalpha, const float* gkl, float* dmu, float* dlogsd,
+                            float* dlogits, void* stream);
+
 /* ---- DKL ----------------------------------------------------------------------
  * Dense Gram K[i][j] = os * k(||(x1_i - x2_j) * inv_ls||), kind 0 = RBF,
  * 1 = Matern-2.5 (gpytorch RBFKernel/MaternKernel/ScaleKernel as configured at
