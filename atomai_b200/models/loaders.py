@@ -21,6 +21,8 @@ def load_model(filepath: str):
         return load_imspec_model(meta)
     if model_type == "vae":
         return load_vae_model(meta)
+    if model_type == "denoising_autoencoder":
+        return load_denoising_autoencoder(meta)
     raise NotImplementedError(f"model_type '{model_type}' is not part of the atomai_b200 hot path")
 
 
@@ -80,4 +82,26 @@ def load_vae_model(meta_dict):
     m.decoder_net.load_state_dict(dec)
     m.decoder_net.eval()
     m.optim = optimizer
+    return m
+
+
+def load_denoising_autoencoder(meta_dict):
+    """Rebuilds a DenoisingAutoencoder (loaders.py:198-235).  The defaults of missing keys are the
+    reference loader's, including use_batch_norm=True where the class itself defaults to False."""
+    from .denoiser import DenoisingAutoencoder
+    meta = dict(meta_dict)
+    meta.pop("model_type", None)
+    weights = meta.pop("weights")
+    optimizer = meta.pop("optimizer", None)
+    m = DenoisingAutoencoder(
+        encoder_filters=meta.pop("encoder_filters", [8, 16, 32, 64]),
+        decoder_filters=meta.pop("decoder_filters", [64, 32, 16, 8]),
+        encoder_layers=meta.pop("encoder_layers", [1, 2, 2, 2]),
+        decoder_layers=meta.pop("decoder_layers", [2, 2, 2, 1]),
+        use_batch_norm=meta.pop("use_batch_norm", True),
+        upsampling_mode=meta.pop("upsampling_mode", 'nearest'),
+        **meta)
+    m.net.load_state_dict(weights)
+    m.net.eval()
+    m.optimizer = optimizer
     return m

@@ -1,4 +1,5 @@
 from .blocks import ConvBlock, DilatedBlock, ResBlock, ResModule, UpsampleBlock
+from .dae import DenoisingAutoencoderNet
 from .ed import (SignalDecoder, SignalED, SignalEncoder, convDecoderNet, convEncoderNet,
                  coord_latent, fcDecoderNet, fcEncoderNet, init_imspec_model, init_VAE_nets,
                  jconvEncoderNet, jfcEncoderNet, rDecoderNet)
@@ -7,7 +8,7 @@ from .gp import (DeepKernel, GPRegressionModel, ScaleToBounds, dense_gram, dense
                  fcFeatureExtractor)
 
 __all__ = ["ConvBlock", "UpsampleBlock", "DilatedBlock", "ResBlock", "ResModule", "Unet", "dilnet",
-           "SegResNet", "ResHedNet", "init_fcnn_model",
+           "SegResNet", "ResHedNet", "init_fcnn_model", "DenoisingAutoencoderNet",
            "SignalEncoder", "SignalDecoder", "SignalED", "convEncoderNet", "convDecoderNet",
            "fcEncoderNet", "fcDecoderNet", "jfcEncoderNet", "jconvEncoderNet", "rDecoderNet", "coord_latent", "init_imspec_model",
            "init_VAE_nets", "fcFeatureExtractor", "DeepKernel", "dense_gram", "dense_rbf",

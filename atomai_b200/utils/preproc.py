@@ -163,6 +163,32 @@ def preprocess_training_imspec_data(X_train, y_train, X_test, y_test, batch_size
     return (*array2list(*tensors, batch_size, memory_alloc), dims)
 
 
+def preprocess_denoiser_data(X_train, y_train, X_test, y_test):
+    """Noisy / clean image pairs -> float32 (n, 1, h, w) tensors (preproc.py:698-758): a
+    channel dimension is added to 3-D inputs with a UserWarning; mixed numpy / torch inputs raise
+    TypeError, noisy / clean shape mismatches ValueError."""
+    data = (X_train, y_train, X_test, y_test)
+    all_np = all(isinstance(i, np.ndarray) for i in data)
+    all_t = all(isinstance(i, torch.Tensor) for i in data)
+    if not all_np and not all_t:
+        raise TypeError(
+            "Provide training and test data in the form of numpy arrays or torch tensors")
+    what = ("noisy training images", "clean training images", "noisy test images",
+            "clean test images")
+    out = []
+    for a, w in zip(data, what):
+        if a.ndim == 3:
+            warnings.warn(f"Adding channel dimension of 1 to {w}", UserWarning)
+            a = a[:, None]
+        out.append(torch.from_numpy(np.ascontiguousarray(a)).float() if all_np else a.float())
+    X_train, y_train, X_test, y_test = out
+    if X_train.shape != y_train.shape:
+        raise ValueError("Noisy and clean training images must have the same shape")
+    if X_test.shape != y_test.shape:
+        raise ValueError("Noisy and clean test images must have the same shape")
+    return X_train, y_train, X_test, y_test
+
+
 def init_dataloaders(X_train, y_train, X_test, y_test, batch_size: int, memory_alloc: float = 4):
     """Train (shuffled) / test DataLoaders over device-resident TensorDatasets, drop_last=True
     (preproc.py:365-388)."""
