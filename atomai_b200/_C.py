@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "libatomai_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
-           "segloss.cu", "refine.cu", "jlatent.cu"]
+           "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -107,6 +107,19 @@ SIGNATURES = {
     "atomai_b200_resize_bwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "atomai_b200_upsample2x_fwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "atomai_b200_upsample2x_bwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "atomai_b200_conv3x3_fwd": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i,
+                                     _i, _vp, _vp]),
+    "atomai_b200_conv3x3_wgrad": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i,
+                                       _i, _vp]),
+    "atomai_b200_dw3x3_dgrad": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "atomai_b200_relu6_bwd_reduce": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i64, _i,
+                                          _i, _vp, _vp]),
+    "atomai_b200_affine_relu6": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i64, _i, _vp]),
+    "atomai_b200_avgpool_relu6_fwd": (_i, [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "atomai_b200_avgpool_bwd": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "atomai_b200_log_softmax_fwd": (_i, [_vp, _vp, _i, _i, _vp]),
+    "atomai_b200_log_softmax_bwd": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
+    "atomai_b200_nll_fwd_bwd": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_transpose": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "atomai_b200_add_slice": (_i, [_vp, _i, _vp, _i, _i, _i64, _i, _vp]),
     "atomai_b200_dilated_sum": (_i, [C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _i, _f, _vp,

@@ -52,14 +52,24 @@ class _CEFn(torch.autograd.Function):
         return gl, None
 
 
+def _dense_layout(t: torch.Tensor) -> bool:
+    """The elements fill their storage span without gaps or overlaps (any dimension order)."""
+    dims = sorted((st, sz) for st, sz in zip(t.stride(), t.shape) if sz > 1)
+    expect = 1
+    for st, sz in dims:
+        if st != expect:
+            return False
+        expect *= sz
+    return True
+
+
 class _PointwiseFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, target, kind):
         if not pred.is_cuda:
             raise RuntimeError("atomai_b200 losses run on CUDA (sm_90a) only")
         # elementwise: memory order is irrelevant as long as both operands share it
-        if pred.stride() == target.stride() and pred.is_non_overlapping_and_dense() \
-                and target.is_non_overlapping_and_dense():
+        if pred.stride() == target.stride() and _dense_layout(pred) and _dense_layout(target):
             p, t = pred.detach(), target.detach()
         else:
             p, t = pred.detach().contiguous(), target.detach().contiguous()
@@ -211,6 +221,38 @@ class MSELoss(torch.nn.MSELoss):
         if self.reduction != "mean":
             raise NotImplementedError("native MSELoss supports reduction='mean' only")
         return _PointwiseFn.apply(input, target, 0)
+
+
+class _NLLFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logp, target):
+        if not logp.is_cuda:
+            raise RuntimeError("atomai_b200 losses run on CUDA (sm_90a) only")
+        if logp.dim() != 2 or target.shape != (logp.shape[0],):
+            raise NotImplementedError("native NLLLoss takes (N, C) log-probabilities and (N,) "
+                                      "targets")
+        lp = logp.detach().float().contiguous()
+        tgt = target.detach().long().contiguous()
+        loss = torch.empty(1, device=lp.device, dtype=torch.float32)
+        ops.nll_fwd_bwd(lp, tgt, loss)
+        ctx.save_for_backward(lp, tgt)
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        lp, tgt = ctx.saved_tensors
+        d = torch.empty_like(lp)
+        ops.nll_fwd_bwd(lp, tgt, None, d, g.detach().float().reshape(1).contiguous())
+        return d, None
+
+
+class NLLLoss(torch.nn.NLLLoss):
+    """Mean negative log-likelihood of (N, C) log-probabilities (the Classifier's criterion,
+    atomai/trainers/trainer.py:929); fused fwd / bwd kernels."""
+    def forward(self, input, target):
+        if self.weight is not None or self.ignore_index != -100 or self.reduction != "mean":
+            raise NotImplementedError("native NLLLoss supports the default options only")
+        return _NLLFn.apply(input, target)
 
 
 def select_loss(loss: str, nb_classes: int = None, **kwargs):

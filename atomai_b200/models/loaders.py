@@ -23,6 +23,10 @@ def load_model(filepath: str):
         return load_vae_model(meta)
     if model_type == "denoising_autoencoder":
         return load_denoising_autoencoder(meta)
+    if model_type == "reg":
+        return load_reg_model(meta)
+    if model_type == "cls":
+        return load_cls_model(meta)
     raise NotImplementedError(f"model_type '{model_type}' is not part of the atomai_b200 hot path")
 
 
@@ -105,3 +109,44 @@ def load_denoising_autoencoder(meta_dict):
     m.net.eval()
     m.optimizer = optimizer
     return m
+
+
+def _regcls_kwargs(meta: dict) -> dict:
+    # the checkpoint stores the image channels as 'in_channels'; the constructor takes
+    # 'input_channels'
+    meta.pop("model_type", None)
+    if "in_channels" in meta:
+        meta["input_channels"] = meta.pop("in_channels")
+    return meta
+
+
+def load_reg_model(meta_dict):
+    """Rebuilds a Regressor from a 'reg' checkpoint (atomai/models/loaders.py:115-137)."""
+    from .regcls import Regressor
+    meta = _regcls_kwargs(dict(meta_dict))
+    backbone = meta.pop("backbone")
+    out_dim = meta.pop("out_dim")
+    weights = meta.pop("weights")
+    optimizer = meta.pop("optimizer", None)
+    model = Regressor(backbone, out_dim, **meta)
+    model.net.load_state_dict(weights)
+    if optimizer is not None:
+        model.optimizer = optimizer
+    model.net.eval()
+    return model
+
+
+def load_cls_model(meta_dict):
+    """Rebuilds a Classifier from a 'cls' checkpoint (atomai/models/loaders.py:140-160)."""
+    from .regcls import Classifier
+    meta = _regcls_kwargs(dict(meta_dict))
+    backbone = meta.pop("backbone")
+    nb_classes = meta.pop("nb_classes")
+    weights = meta.pop("weights")
+    optimizer = meta.pop("optimizer", None)
+    model = Classifier(backbone, nb_classes, **meta)
+    model.net.load_state_dict(weights)
+    if optimizer is not None:
+        model.optimizer = optimizer
+    model.net.eval()
+    return model

@@ -229,6 +229,85 @@ def resize_bwd(dy, dx, factor, bilinear=True) -> None:
                                        1 if bilinear else 0, stream_ptr()))
 
 
+def conv3x3_fwd(x, scale, shift, clip, w, depthwise, y, stride, stats=None) -> None:
+    """y = conv3x3(act(x)), pad 1 (MobileNetV2 stem / depthwise), act = [relu6](x*scale + shift)."""
+    N, H, W, Cin = x.shape
+    Cout = y.shape[3]
+    assert w.is_contiguous() and y.shape[1:3] == ((H - 1) // stride + 1, (W - 1) // stride + 1)
+    check(lib().atomai_b200_conv3x3_fwd(ptr(x), _ld(x), ptr(scale), ptr(shift), 1 if clip else 0,
+                                        ptr(w), 1 if depthwise else 0, ptr(y), _ld(y), N, H, W, Cin,
+                                        Cout, stride, ptr(stats), stream_ptr()))
+
+
+def conv3x3_wgrad(dy, x, scale, shift, clip, depthwise, dw, stride) -> None:
+    """dw (OIHW, zeroed) += weight gradient of conv3x3_fwd."""
+    N, H, W, Cin = x.shape
+    assert dw.is_contiguous()
+    check(lib().atomai_b200_conv3x3_wgrad(ptr(dy), _ld(dy), ptr(x), _ld(x), ptr(scale), ptr(shift),
+                                          1 if clip else 0, 1 if depthwise else 0, ptr(dw), N, H, W,
+                                          Cin, dy.shape[3], stride, stream_ptr()))
+
+
+def dw3x3_dgrad(dy, w, dx, stride) -> None:
+    """dx (N, H, W, C) = data gradient of the depthwise conv3x3_fwd w.r.t. its activated input."""
+    N, H, W, Cc = dx.shape
+    assert w.is_contiguous()
+    check(lib().atomai_b200_dw3x3_dgrad(ptr(dy), _ld(dy), ptr(w), ptr(dx), _ld(dx), N, H, W, Cc,
+                                        stride, stream_ptr()))
+
+
+def relu6_bwd_reduce(dy, a, scale, shift, mean, invstd, g, sums, pooled: bool = False) -> None:
+    """g = dy * relu6'(a*scale + shift) and the BatchNorm-backward sums of g.  pooled: dy is the
+    (N, 1, 1, C) gradient of the average pool over a's H*W pixels, spread as dy / (H*W)."""
+    N, H, W, Cc = a.shape
+    if pooled:
+        assert tuple(dy.shape) == (N, 1, 1, Cc)
+    check(lib().atomai_b200_relu6_bwd_reduce(ptr(dy), _ld(dy), ptr(a), _ld(a), ptr(scale),
+                                             ptr(shift), ptr(mean), ptr(invstd), ptr(g), _ld(g),
+                                             N * H * W, Cc, H * W if pooled else 0, ptr(sums),
+                                             stream_ptr()))
+
+
+def affine_relu6(a, scale, shift, y) -> None:
+    N, H, W, Cc = a.shape
+    check(lib().atomai_b200_affine_relu6(ptr(a), _ld(a), ptr(scale), ptr(shift), ptr(y), _ld(y),
+                                         N * H * W, Cc, stream_ptr()))
+
+
+def avgpool_relu6_fwd(a, scale, shift, y) -> None:
+    """y (N, C) = AdaptiveAvgPool2d(1) of relu6(a*scale + shift)."""
+    N, H, W, Cc = a.shape
+    assert y.is_contiguous() and y.numel() == N * Cc
+    check(lib().atomai_b200_avgpool_relu6_fwd(ptr(a), _ld(a), ptr(scale), ptr(shift), ptr(y), N,
+                                              H * W, Cc, stream_ptr()))
+
+
+def avgpool_bwd(dy, g) -> None:
+    N, H, W, Cc = g.shape
+    assert dy.is_contiguous() and dy.numel() == N * Cc
+    check(lib().atomai_b200_avgpool_bwd(ptr(dy), ptr(g), _ld(g), N, H * W, Cc, stream_ptr()))
+
+
+def log_softmax_fwd(x, y) -> None:
+    B, Cc = x.shape
+    assert x.is_contiguous() and y.is_contiguous()
+    check(lib().atomai_b200_log_softmax_fwd(ptr(x), ptr(y), B, Cc, stream_ptr()))
+
+
+def log_softmax_bwd(y, dy, dx) -> None:
+    B, Cc = y.shape
+    assert y.is_contiguous() and dy.is_contiguous() and dx.is_contiguous()
+    check(lib().atomai_b200_log_softmax_bwd(ptr(y), ptr(dy), ptr(dx), B, Cc, stream_ptr()))
+
+
+def nll_fwd_bwd(logp, target, loss=None, dlogp=None, gscale_dev=None) -> None:
+    B, Cc = logp.shape
+    assert logp.is_contiguous() and target.dtype == torch.int64 and target.is_contiguous()
+    assert target.numel() == B
+    check(lib().atomai_b200_nll_fwd_bwd(ptr(logp), ptr(target), B, Cc, ptr(loss), ptr(dlogp),
+                                        ptr(gscale_dev), stream_ptr()))
+
+
 def transpose(x, y, N, R, Cc) -> None:
     """y[n][c][r] = x[n][r][c] (both contiguous)."""
     assert x.is_contiguous() and y.is_contiguous() and x.numel() == y.numel() == N * R * Cc

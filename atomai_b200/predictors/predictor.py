@@ -331,3 +331,53 @@ class Locator:
         bad = ((coordinates[:, 0] > h - e) | (coordinates[:, 0] < e) |
                (coordinates[:, 1] > w - e) | (coordinates[:, 1] < e))
         return coordinates[~bad]
+
+
+class RegPredictor(BasePredictor):
+    """
+    Prediction with a trained regression model (atomai/predictors/predictor.py:398-482):
+    trained_model, output_dim, use_gpu, **verbose.  run(image_data, **num_batches (10), **norm
+    (True)) returns the squeezed (n, output_dim) numpy array.
+    """
+    def __init__(self, trained_model: Type[torch.nn.Module], output_dim: int,
+                 use_gpu: bool = False, **kwargs: str) -> None:
+        super(RegPredictor, self).__init__(trained_model, use_gpu)
+        set_train_rng(1)
+        self.output_dim = output_dim
+        self.verbose = kwargs.get("verbose", True)
+
+    def preprocess(self, image_data: np.ndarray, norm: bool = True) -> torch.Tensor:
+        if image_data.ndim == 2:
+            image_data = image_data[np.newaxis, ...]
+        return torch_format_image(image_data, norm)
+
+    def _forward_all(self, image_data: np.ndarray, **kwargs) -> torch.Tensor:
+        num_batches = kwargs.get("num_batches", 10)
+        image_data = self.preprocess(image_data, kwargs.get("norm", True))
+        return self.batch_predict(image_data, (len(image_data), self.output_dim), num_batches)
+
+    def predict(self, image_data: np.ndarray, **kwargs: int) -> np.ndarray:
+        return self._forward_all(image_data, **kwargs).squeeze().numpy()
+
+    def run(self, image_data: np.ndarray, **kwargs: int) -> np.ndarray:
+        start_time = time.time()
+        prediction = self.predict(image_data, **kwargs)
+        if self.verbose:
+            n_images = 1 if prediction.ndim == 0 else prediction.shape[0]
+            n_images_str = " image was " if n_images == 1 else " images were "
+            print("\n" + str(n_images) + n_images_str + "decoded in approximately "
+                  + str(np.around(time.time() - start_time, decimals=4)) + ' seconds')
+        return prediction
+
+
+class clsPredictor(RegPredictor):
+    """
+    Prediction with a trained classifier (atomai/predictors/predictor.py:485-530): the argmax
+    class of every image, squeezed.
+    """
+    def __init__(self, trained_model: Type[torch.nn.Module], nb_classes: int,
+                 use_gpu: bool = False, **kwargs: str) -> None:
+        super(clsPredictor, self).__init__(trained_model, nb_classes, use_gpu, **kwargs)
+
+    def predict(self, image_data: np.ndarray, **kwargs: int) -> np.ndarray:
+        return torch.argmax(self._forward_all(image_data, **kwargs), 1).squeeze().numpy()

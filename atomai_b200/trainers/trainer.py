@@ -622,3 +622,108 @@ class ImSpecTrainer(BaseTrainer):
             raise AssertionError(
                 "The input/output dimensions of the model must match" +
                 " the height, width and length (for spectra) of training")
+
+
+def _split_if_no_test(X_train, y_train, X_test, y_test, kwargs):
+    if X_test is None or y_test is None:
+        from sklearn.model_selection import train_test_split
+        X_train, X_test, y_train, y_test = train_test_split(
+            X_train, y_train, test_size=kwargs.get("test_size", .15),
+            shuffle=True, random_state=kwargs.get("seed", 1))
+    return X_train, y_train, X_test, y_test
+
+
+class RegTrainer(BaseTrainer):
+    """
+    Trainer for image -> vector regression (atomai/trainers/trainer.py:860-950): out_dim, backbone
+    ('mobilenet'; 'resnet' / 'vgg' raise NotImplementedError) and the kwargs input_channels,
+    seed, batch_seed.  Criterion: mean squared error.
+    """
+    def __init__(self, out_dim: int = 1, backbone: str = "mobilenet", **kwargs) -> None:
+        super(RegTrainer, self).__init__()
+        from ..nets import init_reg_model
+        seed = kwargs.get("seed", 1)
+        kwargs["batch_seed"] = kwargs.get("batch_seed", seed)
+        set_train_rng(seed)
+        self.output_size = out_dim
+        self.criterion = self.get_loss_fn('mse')
+        self.net, self.meta_state_dict = init_reg_model(out_dim, backbone, **kwargs)
+        self.net.to(self.device)
+        self.meta_state_dict["weights"] = self.net.state_dict()
+
+    def set_data(self, X_train, y_train, X_test=None, y_test=None,
+                 **kwargs: Union[float, int]) -> None:
+        """Images (n, c, h, w) or (n, h, w), targets (n, out_dim) or (n,); a train / test split
+        (test_size, seed) when no test set is given; memory_alloc."""
+        from ..utils.preproc import preprocess_training_reg_data, preprocess_training_reg_data_
+        X_train, y_train, X_test, y_test = _split_if_no_test(X_train, y_train, X_test, y_test,
+                                                             kwargs)
+        memory_alloc = kwargs.get("memory_alloc", 4)
+        if self.full_epoch:
+            self.train_loader, self.test_loader = init_dataloaders(
+                *preprocess_training_reg_data_(X_train, y_train, X_test, y_test),
+                self.batch_size, memory_alloc)
+            train_out_dim = self.train_loader.dataset.tensors[1].shape[-1]
+            test_out_dim = self.test_loader.dataset.tensors[1].shape[-1]
+        else:
+            (self.X_train, self.y_train, self.X_test, self.y_test) = preprocess_training_reg_data(
+                X_train, y_train, X_test, y_test, self.batch_size, memory_alloc)
+            train_out_dim, test_out_dim = self.y_train[0].shape[-1], self.y_test[0].shape[-1]
+        self.data_is_set = True
+        if not train_out_dim == test_out_dim == self.output_size:
+            raise AssertionError(
+                "The output dimensions for the training and test data must be" +
+                " equal to the declared output dimensions")
+
+
+class clsTrainer(BaseTrainer):
+    """
+    Trainer for image classification (atomai/trainers/trainer.py:953-1046): nb_classes, backbone
+    ('mobilenet'; 'resnet' / 'vgg' raise NotImplementedError) and the kwargs input_channels,
+    seed, batch_seed.  Criterion: mean NLL of the network's log-probabilities (losses.NLLLoss).
+    """
+    def __init__(self, nb_classes: int, backbone: str = "mobilenet", **kwargs) -> None:
+        super(clsTrainer, self).__init__()
+        from ..nets import init_cls_model
+        seed = kwargs.get("seed", 1)
+        kwargs["batch_seed"] = kwargs.get("batch_seed", seed)
+        set_train_rng(seed)
+        self.nb_classes = nb_classes
+        self.criterion = losses_metrics.NLLLoss()
+        self.net, self.meta_state_dict = init_cls_model(nb_classes, backbone, **kwargs)
+        self.net.to(self.device)
+        if self.device == 'cpu':
+            warnings.warn("No GPU found. atomai_b200 cannot train without an H100 (sm_90a)",
+                          UserWarning)
+        self.meta_state_dict["weights"] = self.net.state_dict()
+
+    def set_data(self, X_train, y_train, X_test=None, y_test=None,
+                 **kwargs: Union[float, int]) -> None:
+        """Images (n, c, h, w) or (n, h, w) and 1-D int64 class labels; a train / test split
+        (test_size, seed) when no test set is given; memory_alloc."""
+        from ..utils.preproc import preprocess_training_cls_data, preprocess_training_cls_data_
+        X_train, y_train, X_test, y_test = _split_if_no_test(X_train, y_train, X_test, y_test,
+                                                             kwargs)
+        # the NLL kernel cannot raise from the device (an out-of-range label gives a NaN loss), so
+        # the labels are checked once here, on the host
+        for what, y in (("training", y_train), ("test", y_test)):
+            lo, hi = int(y.min()), int(y.max())
+            if lo < 0 or hi >= self.nb_classes:
+                raise ValueError(f"{what} labels must lie in [0, {self.nb_classes - 1}] for "
+                                 f"nb_classes={self.nb_classes}, got [{lo}, {hi}]")
+        memory_alloc = kwargs.get("memory_alloc", 4)
+        if self.full_epoch:
+            self.train_loader, self.test_loader = init_dataloaders(
+                *preprocess_training_cls_data_(X_train, y_train, X_test, y_test),
+                self.batch_size, memory_alloc)
+        else:
+            (self.X_train, self.y_train, self.X_test, self.y_test) = preprocess_training_cls_data(
+                X_train, y_train, X_test, y_test, self.batch_size, memory_alloc)
+        self.data_is_set = True
+
+    def accuracy_fn(self, y: torch.Tensor, y_prob: torch.Tensor, *args):
+        """Ratio of correct argmax predictions (atomai/trainers/trainer.py:1039-1046)."""
+        _, predicted = torch.max(y_prob.data, 1)
+        total = y.size(0)
+        correct = (predicted == y).sum().item()
+        return correct / total

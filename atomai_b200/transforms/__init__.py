@@ -1,3 +1,3 @@
-from .imaug import datatransform, imspec_augmentor, seg_augmentor
+from .imaug import datatransform, imspec_augmentor, reg_augmentor, seg_augmentor
 
-__all__ = ["datatransform", "seg_augmentor", "imspec_augmentor"]
+__all__ = ["datatransform", "seg_augmentor", "imspec_augmentor", "reg_augmentor"]

@@ -145,3 +145,28 @@ def imspec_augmentor(in_dim: Tuple[int], out_dim: Tuple[int], **kwargs) -> Optio
         out, _ = datatransform(None, seed, **augdict).run(features[:, 0], None)
         return out[:, None], targets.to("cuda")
     return augmentor
+
+
+def reg_augmentor(**kwargs) -> Optional[Callable]:
+    """Image-only noise augmentation for Regressor / Classifier (atomai/transforms/imaug.py:461-478):
+    gauss_noise, jitter, poisson_noise, contrast, salt_and_pepper, blur, background on the GPU,
+    targets unchanged.  Other augmentation kwargs (custom_transform, zoom, resize, rotation) raise
+    NotImplementedError."""
+    for k in ("custom_transform", "zoom", "resize", "rotation"):
+        if kwargs.get(k):
+            raise NotImplementedError(
+                f"augmentation '{k}' is not implemented for Regressor / Classifier on the GPU path")
+    keys = ["gauss_noise", "jitter", "poisson_noise", "contrast", "salt_and_pepper", "blur",
+            "background"]
+    augdict = {k: kwargs[k] for k in keys if k in kwargs.keys()}
+    if len(augdict) == 0:
+        return None
+    datatransform(None, None, **augdict)
+
+    def augmentor(features, targets, seed):
+        features = features.to("cuda")
+        if features.shape[1] != 1:
+            raise NotImplementedError("reg_augmentor augments single-channel images only")
+        out, _ = datatransform(None, seed, **augdict).run(features[:, 0], None)
+        return out[:, None], targets.to("cuda")
+    return augmentor

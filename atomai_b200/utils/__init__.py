@@ -8,5 +8,6 @@ from .nn import (average_weights, get_downsample_factor, get_nb_classes, gpu_usa
 from .preproc import (array2list, check_image_dims, check_signal_dims, get_array_memsize,
                       init_dataloader, init_dataloaders, init_fcnn_dataloaders,
                       init_imspec_dataloaders, num_classes_from_labels, preprocess_denoiser_data,
+                      preprocess_training_cls_data, preprocess_training_reg_data,
                       preprocess_training_image_data, preprocess_training_imspec_data,
                       shard_batches, torch_format_image, torch_format_spectra)

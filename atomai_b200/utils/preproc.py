@@ -189,6 +189,74 @@ def preprocess_denoiser_data(X_train, y_train, X_test, y_test):
     return X_train, y_train, X_test, y_test
 
 
+def _check_numpy_or_torch(data) -> bool:
+    all_np = all(isinstance(i, np.ndarray) for i in data)
+    all_t = all(isinstance(i, torch.Tensor) for i in data)
+    if not all_np and not all_t:
+        raise TypeError(
+            "Provide training and test data in the form of numpy arrays or torch tensors")
+    return all_np
+
+
+def _image_channel(X_train, X_test):
+    if X_train.ndim == 3:
+        warnings.warn('Adding a channel dimension of 1 to training images', UserWarning)
+        X_train = X_train[:, None]
+    if X_test.ndim == 3:
+        warnings.warn('Adding a channel dimension of 1 to test images', UserWarning)
+        X_test = X_test[:, None]
+    return X_train, X_test
+
+
+def preprocess_training_reg_data_(X_train, y_train, X_test, y_test):
+    """Images (n, c, h, w) or (n, h, w) and targets (n, out_dim) or (n,) -> float32 tensors; the
+    missing channel / target dimension is added with a UserWarning (preproc.py:481-528)."""
+    all_np = _check_numpy_or_torch((X_train, y_train, X_test, y_test))
+    X_train, X_test = _image_channel(X_train, X_test)
+    if y_train.ndim == 1:
+        warnings.warn('Adding a channel dimension of 1 to training targets', UserWarning)
+        y_train = y_train[:, None]
+    if y_test.ndim == 1:
+        warnings.warn('Adding a channel dimension of 1 to test targets', UserWarning)
+        y_test = y_test[:, None]
+    tor = (lambda a: torch.from_numpy(np.ascontiguousarray(a)).float()) if all_np \
+        else (lambda a: a.float())
+    return tor(X_train), tor(y_train), tor(X_test), tor(y_test)
+
+
+def preprocess_training_reg_data(X_train, y_train, X_test, y_test, batch_size: int,
+                                 memory_alloc: float = 4):
+    """preprocess_training_reg_data_ + lists of batches (preproc.py:531-571)."""
+    return array2list(*preprocess_training_reg_data_(X_train, y_train, X_test, y_test),
+                      batch_size, memory_alloc)
+
+
+def preprocess_training_cls_data_(X_train, y_train, X_test, y_test):
+    """Images (n, c, h, w) or (n, h, w) -> float32, labels must be 1-D int64 (TypeError otherwise;
+    preproc.py:613-656)."""
+    all_np = _check_numpy_or_torch((X_train, y_train, X_test, y_test))
+    X_train, X_test = _image_channel(X_train, X_test)
+    if y_train.dtype not in (torch.int64, np.int64):
+        raise TypeError(
+            "Provide training labels as 1D array of integers (numpy.int64 or torch.int64)")
+    if y_test.dtype not in (torch.int64, np.int64):
+        raise TypeError(
+            "Provide test labels as 1D array of integers (numpy.int64 or torch.int64)")
+    if all_np:
+        return (torch.from_numpy(np.ascontiguousarray(X_train)).float(),
+                torch.from_numpy(np.ascontiguousarray(y_train)),
+                torch.from_numpy(np.ascontiguousarray(X_test)).float(),
+                torch.from_numpy(np.ascontiguousarray(y_test)))
+    return X_train.float(), y_train, X_test.float(), y_test
+
+
+def preprocess_training_cls_data(X_train, y_train, X_test, y_test, batch_size: int,
+                                 memory_alloc: float = 4):
+    """preprocess_training_cls_data_ + lists of batches (preproc.py:659-695)."""
+    return array2list(*preprocess_training_cls_data_(X_train, y_train, X_test, y_test),
+                      batch_size, memory_alloc)
+
+
 def init_dataloaders(X_train, y_train, X_test, y_test, batch_size: int, memory_alloc: float = 4):
     """Train (shuffled) / test DataLoaders over device-resident TensorDatasets, drop_last=True
     (preproc.py:365-388)."""

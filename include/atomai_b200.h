@@ -178,6 +178,49 @@ int atomai_b200_resize_fwd(const float* x, int ld_x, float* y, int ld_y, int N, 
                            int factor, int bilinear, void* stream);
 int atomai_b200_resize_bwd(const float* dy, int ld_dy, float* dx, int ld_dx, int N, int h, int w,
                            int C, int factor, int bilinear, void* stream);
+/* MobileNetV2 (Regressor / Classifier backbone, atomai/nets/blocks.py:376-387), mobilenet.cu.
+ * 3x3 convolution, pad 1, stride 1 or 2, output (N, (H-1)/stride+1, (W-1)/stride+1, Cout): dense
+ * (w: Cout x Cin x 3 x 3, the stem) or depthwise (Cin == Cout, w: C x 1 x 3 x 3).  The input is
+ * read as act(x) = [relu6 if clip](x*scale + shift) (scale/shift may be NULL); stats (2*Cout
+ * doubles, zeroed by the caller, may be NULL) receive the BatchNorm sums (sum y, sum y^2) of the
+ * raw output.  wgrad adds sum over pixels of dy * act(x) into dw (zeroed by the caller); dgrad is
+ * the depthwise data gradient w.r.t. act(x) (gather, no atomics).  Every cross-CTA sum is ordered. */
+int atomai_b200_conv3x3_fwd(const float* x, int ld_x, const float* scale, const float* shift,
+                            int clip, const float* w, int depthwise, float* y, int ld_y, int N,
+                            int H, int W, int Cin, int Cout, int stride, double* stats,
+                            void* stream);
+int atomai_b200_conv3x3_wgrad(const float* dy, int ld_dy, const float* x, int ld_x,
+                              const float* scale, const float* shift, int clip, int depthwise,
+                              float* dw, int N, int H, int W, int Cin, int Cout, int stride,
+                              void* stream);
+int atomai_b200_dw3x3_dgrad(const float* dy, int ld_dy, const float* w, float* dx, int ld_dx,
+                            int N, int H, int W, int C, int stride, void* stream);
+/* BatchNorm -> ReLU6 backward, first pass: g = dy * [0 < a*scale + shift < 6] and
+ * sums += (sum g, sum g * (a - mean) * invstd) per channel (2*C doubles); the apply is
+ * atomai_b200_bn_lrelu_bwd on g with slope 1.  hw > 0: dy is the (N, C) gradient of an average
+ * pool over hw pixels per image (row stride ld_dy), read as dy[n][c] / hw at every pixel. */
+int atomai_b200_relu6_bwd_reduce(const float* dy, int ld_dy, const float* a, int ld_a,
+                                 const float* scale, const float* shift, const float* mean,
+                                 const float* invstd, float* g, int ld_g, int64_t npix, int C,
+                                 int hw, double* sums, void* stream);
+/* y = relu6(a*scale + shift) */
+int atomai_b200_affine_relu6(const float* a, int ld_a, const float* scale, const float* shift,
+                             float* y, int ld_y, int64_t npix, int C, void* stream);
+/* y (N, C) = mean over the HW pixels of relu6(a*scale + shift) (AdaptiveAvgPool2d(1)); backward
+ * g (N, HW, C) = dy / HW */
+int atomai_b200_avgpool_relu6_fwd(const float* a, int ld_a, const float* scale, const float* shift,
+                                  float* y, int N, int HW, int C, void* stream);
+int atomai_b200_avgpool_bwd(const float* dy, float* g, int ld_g, int N, int HW, int C,
+                            void* stream);
+/* LogSoftmax(dim=1) of a contiguous (B, C) matrix and its backward dx = dy - exp(y) sum(dy) */
+int atomai_b200_log_softmax_fwd(const float* x, float* y, int B, int C, void* stream);
+int atomai_b200_log_softmax_bwd(const float* y, const float* dy, float* dx, int B, int C,
+                                void* stream);
+/* mean NLL loss of (B, C) log-probabilities and int64 targets: loss (1 float, may be NULL) =
+ * -mean_i logp[i][t_i] (NaN for a target outside [0, C)); dlogp (may be NULL) = -g/B at the
+ * targets, 0 elsewhere, g read from gscale_dev (NULL: 1). */
+int atomai_b200_nll_fwd_bwd(const float* logp, const int64_t* target, int B, int C, float* loss,
+                            float* dlogp, const float* gscale_dev, void* stream);
 /* y[n][c][r] = x[n][r][c]: NHWC <-> NCHW around `x.reshape(-1, C*H*W)` -> nn.Linear
  * (atomai/nets/ed.py:77-79, 284-287, 516-517). */
 int atomai_b200_transpose(const float* x, float* y, int N, int R, int Cc, void* stream);
