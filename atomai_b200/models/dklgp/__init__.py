@@ -1,3 +1,4 @@
 from .dklgpr import dklGPR
+from .gpr import Reconstructor
 
-__all__ = ["dklGPR"]
+__all__ = ["dklGPR", "Reconstructor"]

@@ -9,7 +9,9 @@ Deep-kernel-learning modules (atomai/nets/gp.py:14-60).
     forms a dense Gram: it configures gpytorch's KISS-GP (GridInterpolationKernel) around the same
     ScaleKernel(RBFKernel(ard)) (nets/gp.py:41-46).  gpytorch is not vendored by the reference and
     not installed in this image; GPRegressionModel therefore needs gpytorch at call time and the
-    dense kernel is exposed for the covariance evaluation itself (SURVEY.md §0.6, §8a a15-a16).
+    dense kernel is exposed for the covariance evaluation itself (SURVEY.md §0.6, §8a a15-a16);
+  * CustomGPModel — the Reconstructor's exact GP on the raw inputs (atomai/nets/gp.py:63-128), its
+    predictive mean on the fused Gram-times-vector kernel (atomai_b200/csrc/gpr.cu).
 """
 from typing import Optional
 
@@ -51,10 +53,12 @@ class fcFeatureExtractor(torch.nn.Sequential):
 
 
 def dense_gram(x1: torch.Tensor, x2: torch.Tensor, lengthscale: torch.Tensor,
-               outputscale: float = 1.0, kind: str = "rbf") -> torch.Tensor:
+               outputscale: float = 1.0, kind: str = "rbf", math: Optional[int] = None
+               ) -> torch.Tensor:
     """K[i, j] = outputscale * k(||(x1_i - x2_j) / lengthscale||) with gpytorch's RBFKernel /
     MaternKernel(nu=2.5) + ScaleKernel definitions, as one fused tiled kernel (no n1 x n2 distance
-    matrix in HBM, exponentiation in the epilogue).  Forward only."""
+    matrix in HBM, exponentiation in the epilogue).  Forward only.  `math` (an ops.MATH_* mode)
+    defaults to the library-wide mode of atomai_b200.set_math."""
     assert x1.is_cuda and x1.dtype == torch.float32 and x1.dim() == 2 and x2.dim() == 2
     inv_ls = (1.0 / lengthscale.to(x1.device, torch.float32).reshape(-1)).contiguous()
     if inv_ls.numel() == 1:
@@ -62,7 +66,7 @@ def dense_gram(x1: torch.Tensor, x2: torch.Tensor, lengthscale: torch.Tensor,
     n2 = x2.shape[0]      # row stride padded to 16 B so that the tensor-core path applies
     out = torch.empty((x1.shape[0], -(-n2 // 4) * 4), device=x1.device, dtype=torch.float32)[:, :n2]
     ops.gram(x1.contiguous(), x2.contiguous(), inv_ls, float(outputscale),
-             {"rbf": 0, "matern": 1}[kind], out, engine._MATH["mode"])
+             {"rbf": 0, "matern": 1}[kind], out, engine._MATH["mode"] if math is None else math)
     return out
 
 
@@ -91,22 +95,34 @@ class DeepKernel(torch.nn.Module):
 
 
 class _DenseGramFn(torch.autograd.Function):
-    """K = outputscale * exp(-0.5 * ||(z1 - z2) / ls||^2) with the native Gram kernel forward and
-    its adjoint built from the kernel output: with W = dK * K,
+    """K = outputscale * k(r^2), r^2 = ||(z1 - z2) / ls||^2, with the native Gram kernel forward and
+    its adjoint built from the kernel output: with W = dK * (-2 dK/dr^2),
         dz1 = -(rowsum(W) * z1 - W z2) / ls^2        dz2 = -(colsum(W) * z2 - W^T z1) / ls^2
         dls = sum_ij W_ij (z1_i - z2_j)^2 / ls^3      dos = sum(dK * K) / os
-    (the two n x n x d products run on the library's own GEMM kernel)."""
+    (the two n x n x d products run on the library's own GEMM kernel).  RBF: -2 dK/dr^2 = K.
+    Matern-2.5 (s = sqrt(5) r): -2 dK/dr^2 = 5/3 os (1 + s) exp(-s) = 5/3 K (1 + s) / (1 + s + s^2/3),
+    with r^2 = -2 log(exp(-r^2 / 2)) from the native RBF Gram at unit outputscale (the factor is 0
+    where that underflows, r^2 > ~200, where K / os < e^-31)."""
 
     @staticmethod
-    def forward(ctx, z1, z2, ls, os_):
-        K = dense_gram(z1, z2, ls.detach(), float(os_), "rbf")
+    def forward(ctx, z1, z2, ls, os_, kind="rbf", math=None):
+        K = dense_gram(z1, z2, ls.detach(), float(os_), kind, math)
         ctx.save_for_backward(z1, z2, ls, os_, K)
+        ctx.kind, ctx.math = kind, math
         return K
 
     @staticmethod
     def backward(ctx, dK):
         z1, z2, ls, os_, K = ctx.saved_tensors
-        W = (dK.to(torch.float32) * K).contiguous()
+        if ctx.kind == "rbf":
+            W = (dK.to(torch.float32) * K).contiguous()
+        else:
+            e = dense_gram(z1, z2, ls.detach(), 1.0, "rbf", ctx.math)
+            d2 = -2.0 * torch.log(e)
+            sr = torch.sqrt(5.0 * d2)
+            m = torch.where(e > 0, (5.0 / 3.0) * K * (1.0 + sr) / (1.0 + sr + (5.0 / 3.0) * d2),
+                            torch.zeros_like(K))
+            W = (dK.to(torch.float32) * m).contiguous()
         n1, n2, d = z1.shape[0], z2.shape[0], z1.shape[1]
         z1c, z2c = z1.contiguous(), z2.contiguous()
         Wz2 = torch.empty((n1, d), device=W.device, dtype=torch.float32)
@@ -120,12 +136,18 @@ class _DenseGramFn(torch.autograd.Function):
         s = (rs * z1c * z1c).sum(0) + (cs * z2c * z2c).sum(0) - 2.0 * (z1c * Wz2).sum(0)
         dls = s / (ls * ls * ls)
         dos = (dK * K).sum() / os_
-        return dz1, dz2, dls, dos
+        return dz1, dz2, dls, dos, None, None
 
 
 def dense_rbf(z1, z2, lengthscale, outputscale):
     """Differentiable dense ScaleKernel(RBFKernel(ard)) Gram on the native kernels."""
     return _DenseGramFn.apply(z1, z2, lengthscale, outputscale)
+
+
+def dense_kernel(z1, z2, lengthscale, outputscale, kind: str = "rbf", math: Optional[int] = None):
+    """Differentiable dense ScaleKernel(RBFKernel | MaternKernel(nu=2.5), ard) Gram on the native
+    kernels (`kind` "rbf" | "matern"); `math` as dense_gram."""
+    return _DenseGramFn.apply(z1, z2, lengthscale, outputscale, kind, math)
 
 
 class ScaleToBounds(torch.nn.Module):
@@ -248,3 +270,177 @@ class GPRegressionModel(torch.nn.Module):
             v = torch.linalg.solve_triangular(Ls[b], Ks, upper=False)
             vars_.append((self.outputscale[b].to(y.dtype) - (v * v).sum(0)).clamp_min(1e-10))
         return torch.stack(means), torch.stack(vars_)
+
+
+class _ExactGramFn(torch.autograd.Function):
+    """K + noise I of the exact GP in float64 on the native kernels (atomai_b200_gram_f64: coordinate
+    differences, float64 throughout, so the matrix is symmetric positive definite to float64
+    rounding) and its hyper-parameter adjoint (atomai_b200_gram_f64_adjoint):
+        dls_k = os sum_ij G_ij m_ij t_ijk^2 / ls_k,   dos = sum_ij G_ij k_ij,   dnoise = tr G
+    with t_ijk = (z_ik - z_jk) / ls_k, k the unit-outputscale kernel, m = -2 dk/dr^2."""
+
+    @staticmethod
+    def forward(ctx, z, ls, os_, noise, kind):
+        inv_ls = (1.0 / ls.detach().to(torch.float64)).reshape(-1).contiguous()
+        n = z.shape[0]
+        K = torch.empty((n, n), device=z.device, dtype=torch.float64)
+        ops.gram_f64(z, inv_ls, float(os_), float(noise), _KIND[kind], K)
+        ctx.save_for_backward(z, inv_ls, ls, os_, noise)
+        ctx.kind = kind
+        return K
+
+    @staticmethod
+    def backward(ctx, G):
+        z, inv_ls, ls, os_, noise = ctx.saved_tensors
+        d = z.shape[1]
+        s = torch.empty(d + 2, device=z.device, dtype=torch.float64)
+        ops.gram_f64_adjoint(z, inv_ls, _KIND[ctx.kind], G.contiguous(), s)
+        dls = (os_.detach().to(torch.float64) * s[:d] * inv_ls).to(ls.dtype).reshape(ls.shape)
+        return (None, dls, s[d].to(os_.dtype).reshape(os_.shape),
+                s[d + 1].to(noise.dtype).reshape(noise.shape), None)
+
+
+_KIND = {"rbf": 0, "matern": 1}
+
+
+class CustomGPModel(torch.nn.Module):
+    """
+    Exact GP of the Reconstructor (atomai/nets/gp.py:63-128): ConstantMean + ScaleKernel(RBFKernel |
+    MaternKernel(nu=2.5), ARD) on the raw inputs, Gaussian likelihood.  The reference wraps the base
+    kernel in gpytorch's KISS-GP (GridInterpolationKernel); here the Gram is evaluated densely on
+    the native kernels and the GP algebra is a float64 Cholesky (torch.linalg) — an exact GP in
+    place of the SKI approximation of it, so `grid_points_ratio` is accepted and ignored.
+
+    The hyper-parameters restate gpytorch's parametrisation (gpytorch is a third-party dependency
+    of the reference, not vendored and not installed here, so the restatement is not checked
+    against it):
+      lengthscale = softplus(raw), or with `lengthscale_constraints` = (lower, upper) gpytorch's
+                    Interval: lower + (upper - lower) * sigmoid(raw); raw starts at 0 either way
+                    (an Interval without an initial value leaves the raw parameter alone, so the
+                    lengthscale starts at the midpoint);
+      outputscale = softplus(raw), noise = softplus(raw) + 1e-4, mean constant = raw; all raw
+                    values start at 0.
+    The raw parameters are float32 (the native Adam updates them); the training Gram, its adjoint
+    and the algebra are float64 (_ExactGramFn), the predictive mean is summed in float64.
+    """
+    def __init__(self, train_x: torch.Tensor, train_y: torch.Tensor, likelihood=None,
+                 kernel_type: str = "kissgp", base_kernel="rbf", inducing_points=None,
+                 grid_points_ratio: float = 1.0, lengthscale_constraints=None, **kwargs):
+        super().__init__()
+        if isinstance(base_kernel, str):
+            if base_kernel not in ("rbf", "matern"):
+                raise ValueError("base_kernel must be either 'rbf', 'matern', or a custom "
+                                 "gpytorch.kernels.Kernel object")
+        else:
+            raise NotImplementedError("custom base kernel objects are not supported: the native "
+                                      "Gram kernels implement 'rbf' and 'matern' (nu=2.5) only")
+        if kernel_type == "sparse":
+            raise NotImplementedError("kernel_type='sparse' (inducing-point kernel) is not "
+                                      "implemented; use kernel_type='kissgp' (exact GP)")
+        if kernel_type != "kissgp":
+            raise ValueError(f"Invalid kernel_type: {kernel_type}. "
+                             "Supported values are 'sparse' and 'kissgp'.")
+        if inducing_points is not None:
+            raise NotImplementedError("inducing_points belong to the sparse kernel, which is not "
+                                      "implemented")
+        d = train_x.shape[-1]
+        if not 1 <= d <= 4:
+            raise NotImplementedError(f"the native GP mean kernel takes 1 to 4 input dimensions, "
+                                      f"got {d}")
+        self.kind = base_kernel
+        self.train_inputs = (train_x,)
+        self.train_targets = train_y.reshape(-1)
+        self.raw_constant = torch.nn.Parameter(torch.zeros(()))
+        self.raw_lengthscale = torch.nn.Parameter(torch.zeros(1, d))
+        self.raw_outputscale = torch.nn.Parameter(torch.zeros(()))
+        self.raw_noise = torch.nn.Parameter(torch.zeros(1))
+        self.interval = lengthscale_constraints is not None and len(lengthscale_constraints) > 0
+        lo, hi = (lengthscale_constraints if self.interval else ([0.0] * d, [0.0] * d))
+        self.register_buffer("ls_lower", torch.as_tensor(lo, dtype=torch.float32).reshape(-1))
+        self.register_buffer("ls_upper", torch.as_tensor(hi, dtype=torch.float32).reshape(-1))
+        if self.interval and not bool((self.ls_lower < self.ls_upper).all()):
+            raise ValueError("Got parameter bounds with empty intervals.")
+        self.likelihood = likelihood
+        self._cache = None
+
+    @property
+    def lengthscale(self) -> torch.Tensor:
+        if self.interval:
+            return self.ls_lower + (self.ls_upper - self.ls_lower) * torch.sigmoid(self.raw_lengthscale)
+        return torch.nn.functional.softplus(self.raw_lengthscale)
+
+    @property
+    def outputscale(self) -> torch.Tensor:
+        return torch.nn.functional.softplus(self.raw_outputscale)
+
+    @property
+    def noise(self) -> torch.Tensor:
+        return torch.nn.functional.softplus(self.raw_noise) + 1e-4
+
+    @property
+    def constant(self) -> torch.Tensor:
+        return self.raw_constant
+
+    def covar_parameters(self):
+        return [self.raw_lengthscale, self.raw_outputscale]
+
+    def mean_parameters(self):
+        return [self.raw_constant]
+
+    def likelihood_parameters(self):
+        return [self.raw_noise]
+
+    def _inputs64(self, x: torch.Tensor) -> torch.Tensor:
+        # coordinates relative to the rounded training mean: the distances are unchanged, integer
+        # pixel indices stay integers (exact in fp32 for the mean kernel) and small
+        return (x.to(torch.float64) - self._center).contiguous()
+
+    def _inputs(self, x: torch.Tensor) -> torch.Tensor:
+        return self._inputs64(x).to(torch.float32).contiguous()
+
+    def _set_center(self) -> None:
+        self._center = self.train_inputs[0].to(torch.float64).mean(0).round()
+
+    def neg_mll(self) -> torch.Tensor:
+        """-ExactMarginalLogLikelihood / N (gpytorch divides by the number of data points), the
+        loss of GPTrainer.train_step (atomai/trainers/gptrainer.py:126-137)."""
+        self._cache = None
+        self._set_center()
+        z = self._inputs64(self.train_inputs[0])
+        n = z.shape[0]
+        Kn = _ExactGramFn.apply(z, self.lengthscale.reshape(-1), self.outputscale, self.noise,
+                                self.kind)
+        L = torch.linalg.cholesky(Kn)
+        del Kn
+        r = (self.train_targets.to(torch.float64) - self.constant.to(torch.float64))[:, None]
+        alpha = torch.cholesky_solve(r, L)
+        mll = -0.5 * (r * alpha).sum() - torch.log(torch.diagonal(L)).sum() \
+            - 0.5 * n * 1.8378770664093453
+        return -mll / n
+
+    @torch.no_grad()
+    def _weights(self):
+        if self._cache is None:
+            self._set_center()
+            z = self._inputs64(self.train_inputs[0])
+            n = z.shape[0]
+            ls = self.lengthscale.reshape(-1)
+            K = torch.empty((n, n), device=z.device, dtype=torch.float64)
+            ops.gram_f64(z, (1.0 / ls.to(torch.float64)).contiguous(), float(self.outputscale),
+                         float(self.noise), _KIND[self.kind], K)
+            L = torch.linalg.cholesky(K)
+            del K
+            r = (self.train_targets.to(torch.float64) - self.constant.to(torch.float64))[:, None]
+            alpha = torch.cholesky_solve(r, L).reshape(-1).contiguous()
+            self._cache = (z.to(torch.float32).contiguous(), (1.0 / ls).contiguous(), alpha)
+        return self._cache
+
+    @torch.no_grad()
+    def posterior_mean(self, x_new: torch.Tensor) -> torch.Tensor:
+        """Predictive mean at x_new ((n, d)) as float64, from the fused Gram-times-vector kernel
+        (the n x N cross-Gram is never formed)."""
+        z, inv_ls, alpha = self._weights()
+        out = torch.empty(x_new.shape[0], device=z.device, dtype=torch.float64)
+        ops.gram_matvec(self._inputs(x_new.to(z.device)), z, inv_ls, alpha, float(self.constant.detach()),
+                        float(self.outputscale), _KIND[self.kind], out)
+        return out

@@ -490,6 +490,39 @@ def gram(x1, x2, inv_ls, outputscale, kind, out, math=MATH_TF32X3) -> None:
                                  stream_ptr()))
 
 
+def gram_matvec(xq, x, inv_ls, alpha, c, outputscale, kind, out) -> None:
+    """out[i] = c + outputscale * sum_j k(||(xq_i - x_j) * inv_ls||) alpha_j without forming the
+    cross-Gram: xq (nq, d), x (n, d), inv_ls (d,) fp32; alpha (n,), out (nq,) float64; d <= 4."""
+    nq, d = xq.shape
+    n = x.shape[0]
+    assert xq.dtype == x.dtype == inv_ls.dtype == torch.float32 and x.shape[1] == d
+    assert alpha.dtype == out.dtype == torch.float64 and alpha.numel() == n and out.numel() == nq
+    assert all(t.is_contiguous() for t in (xq, x, inv_ls, alpha, out)) and inv_ls.numel() == d
+    check(lib().atomai_b200_gram_matvec(ptr(xq), ptr(x), ptr(inv_ls), ptr(alpha), float(c),
+                                        float(outputscale), nq, n, d, kind, ptr(out),
+                                        stream_ptr()))
+
+
+def gram_f64(x, inv_ls, outputscale, noise, kind, out) -> None:
+    """out (n, n) float64 <- outputscale * k(||(x_i - x_j) * inv_ls||) + noise on the diagonal;
+    x (n, d) and inv_ls (d,) float64, d <= 4."""
+    n, d = x.shape
+    assert x.dtype == inv_ls.dtype == out.dtype == torch.float64 and inv_ls.numel() == d
+    assert x.is_contiguous() and inv_ls.is_contiguous() and out.shape == (n, n) and out.stride(1) == 1
+    check(lib().atomai_b200_gram_f64(ptr(x), ptr(inv_ls), float(outputscale), float(noise), n, d,
+                                     kind, ptr(out), out.stride(0), stream_ptr()))
+
+
+def gram_f64_adjoint(x, inv_ls, kind, G, out) -> None:
+    """out (d + 2,) float64 <- [sum G m t_k^2 (k < d), sum G k, trace G] for the Gram of gram_f64
+    at unit outputscale (see include/atomai_b200.h)."""
+    n, d = x.shape
+    assert G.dtype == out.dtype == torch.float64 and G.shape == (n, n) and G.stride(1) == 1
+    assert x.is_contiguous() and inv_ls.is_contiguous() and out.numel() == d + 2
+    check(lib().atomai_b200_gram_f64_adjoint(ptr(x), ptr(inv_ls), n, d, kind, ptr(G), G.stride(0),
+                                             ptr(out), stream_ptr()))
+
+
 def prob_mask(logits_nhwc, mode: int, thresh: float, prob, mask=None) -> None:
     """prob = softmax (mode 0) / sigmoid (1) / exp (2) / identity (3) of NHWC logits; mask (uint8,
     optional) = prob > thresh."""

@@ -12,7 +12,7 @@ from typing import Optional, Tuple, Type, Union
 import numpy as np
 import torch
 
-from ..nets.gp import GPRegressionModel, fcFeatureExtractor
+from ..nets.gp import CustomGPModel, GPRegressionModel, fcFeatureExtractor
 from ..optim import FusedAdam
 
 
@@ -24,6 +24,26 @@ def set_seed_and_precision(seed: int = 42, precision: str = "double", **kwargs) 
     torch.manual_seed(seed)
     if torch.cuda.is_available():
         torch.cuda.manual_seed_all(seed)
+
+
+# float64 N x N matrices counted for an exact-GP training step: the measured peak is 6.0 (the
+# Cholesky factor - K + noise is freed once factored - and the temporaries of the cholesky_solve and
+# Cholesky backward passes up to the gradient of K + noise, which the adjoint kernel reads in
+# place) plus O(N) vectors; one more matrix of headroom for the allocator's rounding
+# (tests/test_reconstructor_gpu.py measures the peak against this count)
+_EXACT_GP_NXN = 7
+
+
+def check_exact_gp_memory(n: int, device) -> None:
+    """Fails before anything is allocated when the float64 N x N algebra of an exact GP on n
+    points cannot fit in the free memory of `device`."""
+    need = _EXACT_GP_NXN * 8 * n * n
+    free, _ = torch.cuda.mem_get_info(torch.device(device))
+    if need > free:
+        raise MemoryError(
+            f"exact GP on N = {n} points needs about {need / 2**30:.1f} GiB for its float64 "
+            f"N x N Cholesky algebra, {free / 2**30:.1f} GiB of device memory are free; "
+            "measure fewer points (a sparser scan or a crop)")
 
 
 class GPTrainer:
@@ -54,6 +74,36 @@ class GPTrainer:
             y = y[None] if y.ndim == 1 else y
             y = self._set_data(y, device)
         return x, y
+
+    def compile_trainer(self, X, y, training_cycles: int = 1, **kwargs) -> None:
+        """Exact GP on the raw inputs (atomai/trainers/gptrainer.py:59-93): CustomGPModel with the
+        kwargs kernel_type, base_kernel, inducing_points, grid_points_ratio (ignored: the GP is
+        exact), lengthscale_constraints; Adam over every hyper-parameter with kwargs lr (0.1)."""
+        X, y = self.set_data(X, y)
+        self.gp_model = CustomGPModel(X, y, None, **kwargs)
+        if not str(self.device).startswith("cuda"):
+            raise RuntimeError("atomai_b200 runs on CUDA (H100, sm_90a) only: the native GP "
+                               "kernels have no CPU fallback")
+        check_exact_gp_memory(X.shape[0], self.device)
+        self.gp_model.to(self.device)
+        self.gp_model.train()
+        list_of_params = [{'params': self.gp_model.covar_parameters()},
+                          {'params': self.gp_model.mean_parameters()},
+                          {'params': self.gp_model.likelihood_parameters()}]
+        self.optimizer = FusedAdam(list_of_params, lr=kwargs.get("lr", 0.1))
+        self.training_cycles = training_cycles
+        self.compiled = True
+
+    def run(self, X=None, y=None, training_cycles: int = 1, **kwargs):
+        """Initializes (if needed) and trains the GP (atomai/trainers/gptrainer.py:95-124)."""
+        if not self.compiled:
+            self.compile_trainer(X, y, training_cycles, **kwargs)
+        for e in range(self.training_cycles):
+            self.train_step()
+            if any([e == 0, (e + 1) % kwargs.get("print_loss", 10) == 0,
+                    e == self.training_cycles - 1]):
+                self.print_statistics(e)
+        return self.gp_model
 
     def train_step(self) -> None:
         """Full-batch step on -mll (atomai/trainers/gptrainer.py:126-137)."""

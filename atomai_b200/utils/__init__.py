@@ -1,13 +1,14 @@
-from .coords import (find_com, get_nn_distances_, grid2xy, imcoordgrid, peak_refinement,
-                     remove_edge_coord, transform_coordinates)
+from .coords import (find_com, get_lengthscale_constraints, get_nn_distances_, grid2xy,
+                     imcoordgrid, peak_refinement, remove_edge_coord, transform_coordinates)
 from .img import (crop_borders, cv_thresh, extract_random_subimages, extract_subimages,
                   extract_subimages_cuda, get_coord_grid,
                   get_imgstack, imcrop_randcoord, imcrop_randpx, img_pad, img_resize)
 from .nn import (average_weights, get_downsample_factor, get_nb_classes, gpu_usage_map,
                  mock_forward, reset_bnorm, sample_weights, set_train_rng, weights_init)
-from .preproc import (array2list, check_image_dims, check_signal_dims, get_array_memsize,
+from .preproc import (array2list, check_image_dims, check_signal_dims, create_batches,
+                      get_array_memsize,
                       init_dataloader, init_dataloaders, init_fcnn_dataloaders,
                       init_imspec_dataloaders, num_classes_from_labels, preprocess_denoiser_data,
-                      preprocess_training_cls_data, preprocess_training_reg_data,
+                      prepare_gp_input, preprocess_training_cls_data, preprocess_training_reg_data,
                       preprocess_training_image_data, preprocess_training_imspec_data,
                       shard_batches, torch_format_image, torch_format_spectra)

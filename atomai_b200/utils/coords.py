@@ -209,3 +209,10 @@ def peak_refinement(imgdata: Union[np.ndarray, torch.Tensor], coordinates: np.nd
     """
     stack = imgdata[None] if isinstance(imgdata, torch.Tensor) else np.asarray(imgdata)[None]
     return refine_frames(stack, [np.asarray(coordinates)], d)[0]
+
+
+def get_lengthscale_constraints(grid: np.ndarray) -> list:
+    """[lower, upper] lengthscale bounds for a GP on the pixel grid `grid` ((N, ndim) indices):
+    1 and half the largest index + 1 per dimension (atomai/utils/coords.py:540-543)."""
+    upper = np.amax(grid, axis=0) // 2 + 1
+    return [np.ones(grid.shape[-1]).tolist(), upper.tolist()]

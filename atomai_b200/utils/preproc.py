@@ -327,3 +327,24 @@ def shard_batches(batches: List[torch.Tensor], rank: int, world: int) -> List[to
         k = n // world
         out.append(b[rank * k:(rank + 1) * k].contiguous())
     return out
+
+
+def create_batches(array, batch_size: int) -> list:
+    """Consecutive slices of `batch_size` rows of an array / tensor, the last one possibly shorter
+    (atomai/utils/preproc.py:932-935)."""
+    nb = -(-array.shape[0] // batch_size)
+    return [array[k * batch_size:(k + 1) * batch_size] for k in range(nb)]
+
+
+def prepare_gp_input(sparse_image: np.ndarray):
+    """GP inputs of a sparse scan whose unmeasured pixels are zero (atomai/utils/preproc.py:938-947):
+    the indices (N, ndim) of the non-zero pixels in row-major order, their values (N,), and the
+    indices of every pixel (H*W..., ndim).  The full grid is numpy's meshgrid (default 'xy'
+    indexing) stacked and transposed, whose rows for a 2-D image run in row-major order, so a
+    prediction over it reshapes back into the image."""
+    measured = np.nonzero(sparse_image)
+    x_train = np.stack(measured, axis=1)
+    y_train = sparse_image[measured]
+    axes = [np.arange(n) for n in sparse_image.shape]
+    x_full = np.array(np.meshgrid(*axes)).T.reshape(-1, sparse_image.ndim)
+    return x_train, y_train, x_full

@@ -375,6 +375,28 @@ int64_t atomai_b200_gram_workspace_bytes(int n1, int n2, int d);
 int atomai_b200_gram(const float* x1, const float* x2, const float* inv_ls, float outputscale,
                      int n1, int n2, int d, int kind, int math, float* K, int64_t ldk,
                      void* workspace, int64_t workspace_bytes, void* stream);
+/* GP predictive mean without the cross-Gram (csrc/gpr.cu):
+ *   y[i] = c + outputscale * sum_j k(||(xq_i - x_j) * inv_ls||) * alpha_j
+ * for nq query points xq: [nq][d] against n training points x: [n][d] (fp32, row-major),
+ * inv_ls: [d], 1 <= d <= 4, kind as atomai_b200_gram.  alpha: [n] and y: [nq] are double.  k is
+ * evaluated in fp32 from the coordinate differences; each y[i] is accumulated in double in a fixed
+ * order of j that does not depend on nq, so a query gets identical bits however the queries are
+ * batched.  The nq x n matrix is never formed. */
+int atomai_b200_gram_matvec(const float* xq, const float* x, const float* inv_ls,
+                            const double* alpha, double c, double outputscale, int nq, int n, int d,
+                            int kind, double* y, void* stream);
+/* Exact-GP training Gram in double (csrc/gpr.cu): K[i][j] = outputscale * k(||(x_i - x_j) * inv_ls||)
+ * + noise [i == j] for x: [n][d] double, 1 <= d <= 4, kind as atomai_b200_gram, from coordinate
+ * differences (exactly symmetric, no norm-expansion cancellation).  K: [n][ldk] double. */
+int atomai_b200_gram_f64(const double* x, const double* inv_ls, double outputscale, double noise,
+                         int n, int d, int kind, double* K, int64_t ldk, void* stream);
+/* Its adjoint for an upstream gradient G: [n][ldg] double, with t_ijk = (x_ik - x_jk) inv_ls_k,
+ * k_ij = k(r_ij^2) and m_ij = -2 dk/dr^2 (RBF: k; Matern-2.5: 5/3 (1 + s) exp(-s)):
+ * out[k] = sum_ij G_ij m_ij t_ijk^2 (k < d), out[d] = sum_ij G_ij k_ij, out[d + 1] = sum_i G_ii,
+ * i.e. dL/dls_k = os out[k] / ls_k, dL/dos = out[d], dL/dnoise = out[d + 1].  Double sums in a
+ * fixed order (bit-identical on repeat). */
+int atomai_b200_gram_f64_adjoint(const double* x, const double* inv_ls, int n, int d, int kind,
+                                 const double* G, int64_t ldg, double* out, void* stream);
 
 /* ---- prediction front-end / data path (SURVEY.md 8f) -----------------------------
  * prob[p][c] = softmax_c(logits[p][:]) (mode 0) | sigmoid (1) | exp (2) | identity (3) over NHWC
