@@ -141,6 +141,31 @@ __device__ __forceinline__ void mbar_wait_quiet(uint32_t bar, uint32_t parity) {
     }
   }
 }
+// consumer warp of a stage ring: every warp of the group arrives once it has seen its MMAs retire
+// (bar = 0: nothing to release)
+__device__ __forceinline__ void consumer_release(uint32_t bar) {
+  if (bar) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+  }
+}
+// named barriers: id 0 is __syncthreads, n = participating threads (a multiple of 32)
+__device__ __forceinline__ void named_bar_sync(int id, int n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int n) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+// Warp-specialised kernels are launched at one register count and move registers between their
+// warpgroups: every warp of the warpgroup executes the same call (.sync.aligned).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
 __device__ __forceinline__ void prefetch_l2(const void* p) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }

@@ -102,22 +102,8 @@ struct __align__(8) SharedCtl {
   unsigned red_last;
 };
 
-// consumer warp: every warp of the group arrives once it has seen its MMAs retire
-__device__ __forceinline__ void consumer_release(uint32_t bar) {
-  if (bar) {
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
-  }
-}
-
 // named barriers (id 0 = __syncthreads, 1 = the consumers' final statistics sum)
 constexpr int kStatBar = 2;   // 2..5: consumer 0 -> 1 statistics token of warp w, 6..9: 1 -> 0
-__device__ __forceinline__ void named_bar_sync(int id, int n) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
-}
-__device__ __forceinline__ void named_bar_arrive(int id, int n) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
-}
 
 // Streamed-weight refill issued by one thread of a consumer warpgroup.  The copies are predicated
 // instead of branched on: a divergent branch while MMAs are in flight makes ptxas serialise them.
@@ -739,7 +725,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   __syncthreads();
 
   if (warp >= kFirstLoadWarp) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegsLoad));
+    setmaxnreg_dec<kRegsLoad>();
     // ===================== activation loaders =====================
     // Two groups of 4 warps; group g stages every k-chunk of the tiles with local index = g
     // (mod 2), so two chunks are always in flight per SM.  Per thread the (halo row, halo col) of
@@ -770,10 +756,10 @@ __global__ void __launch_bounds__(kThreads, 1)
     // one branch per consumer ahead of setmaxnreg (.sync.aligned: each warpgroup is converged
     // after it), so nothing in a consumer's wgmma code depends on the thread index
     if (warp < kNumEpiWarps) {
-      asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsCons));
+      setmaxnreg_inc<kRegsCons>();
       conv_consumer<0>(p, ctl, a_base, b_base, s_stats, s_bias);
     } else {
-      asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegsCons));
+      setmaxnreg_inc<kRegsCons>();
       conv_consumer<1>(p, ctl, a_base, b_base, s_stats, s_bias);
     }
   }
