@@ -8,8 +8,8 @@ convolutions + HBM-bound fused kernels); there is no CPU or eager-PyTorch fallba
 """
 from .__version__ import version as __version__
 from .engine import get_math, set_fusion, set_math
-from . import losses_metrics, models, nets, predictors, trainers, transforms, utils
+from . import losses_metrics, models, nets, predictors, stat, trainers, transforms, utils
 
-__all__ = ["nets", "losses_metrics", "trainers", "predictors", "models", "utils", "transforms",
+__all__ = ["nets", "losses_metrics", "trainers", "predictors", "models", "utils", "transforms", "stat",
            "set_math", "set_fusion",
            "get_math", "__version__"]

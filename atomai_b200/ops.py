@@ -541,6 +541,71 @@ def gather_windows(img_nhwc, table, r: int, out, nanflag=None) -> None:
                                            ptr(out), ptr(nanflag), stream_ptr()))
 
 
+STAT_GMM, STAT_KMEANS, STAT_KPP = 0, 1, 2
+
+
+def _stat_math(math):
+    from .engine import _MATH
+    return _MATH["mode"] if math is None else math
+
+
+def stat_estep(X, mu, mode, A, B, cst, out, closest=None, resp=None, labels=None, rowval=None,
+               D=None, changes=None, math=None) -> None:
+    """One pass over the fp32 (N, d) X centred by mu: GMM responsibilities / k-means assignment /
+    k-means++ candidate potentials (see include/atomai_b200.h); out is float64.  `math`
+    (MATH_*, default: the set_math mode) picks the wgmma or the exact-FFMA kernel."""
+    N, d = X.shape
+    K = A.shape[0]
+    assert X.is_contiguous() and X.dtype == torch.float32 and A.shape == (K, d)
+    assert out.dtype == torch.float64
+    check(lib().atomai_b200_stat_estep(ptr(X), ptr(mu), N, d, K, mode, ptr(A), ptr(B), ptr(cst),
+                                       ptr(closest), ptr(resp), ptr(labels), ptr(rowval), ptr(D),
+                                       ptr(out), ptr(changes), _stat_math(math), stream_ptr()))
+
+
+def stat_accum(X, mu, K, sx, sxx=None, nk=None, resp=None, labels=None, math=None) -> None:
+    """float64 sx (K, d) = sum_n r_nk (x_n - mu), sxx likewise of the squares, nk = sum_n r_nk, with
+    r = resp (N, K) fp32, else one-hot int32 labels, else all rows in component 0; `math` as in
+    stat_estep."""
+    N, d = X.shape
+    assert X.is_contiguous() and X.dtype == torch.float32 and sx.shape == (K, d)
+    check(lib().atomai_b200_stat_accum(ptr(X), ptr(mu), N, d, K, ptr(resp), ptr(labels), ptr(sx),
+                                       ptr(sxx), ptr(nk), _stat_math(math), stream_ptr()))
+
+
+def stat_gmm_params(sx, sxx, nk, N, spherical, reg_covar, init, means, covs, weights, A, B, cst):
+    K, d = sx.shape
+    check(lib().atomai_b200_stat_gmm_params(ptr(sx), ptr(sxx), ptr(nk), N, d, K, int(spherical),
+                                            float(reg_covar), int(init), ptr(means), ptr(covs),
+                                            ptr(weights), ptr(A), ptr(B), ptr(cst), stream_ptr()))
+
+
+def stat_kmeans_centres(c_new, A, cst, sx=None, nk=None, c_old=None, shift=None) -> None:
+    K, d = c_new.shape
+    check(lib().atomai_b200_stat_kmeans_centres(ptr(sx), ptr(nk), ptr(c_old), ptr(c_new), K, d,
+                                                ptr(A), ptr(cst), ptr(shift), stream_ptr()))
+
+
+def stat_kpp_chunks(N: int) -> int:
+    return int(lib().atomai_b200_stat_kpp_chunks(N))
+
+
+def stat_kpp_candidates(closest, N, ntr, seed, counter, chunk_ws, idx) -> None:
+    check(lib().atomai_b200_stat_kpp_candidates(ptr(closest), N, ntr, seed, counter, ptr(chunk_ws),
+                                                ptr(idx), stream_ptr()))
+
+
+def stat_gather_rows(X, mu, idx, out) -> None:
+    check(lib().atomai_b200_stat_gather_rows(ptr(X), ptr(mu), X.shape[1], ptr(idx), idx.numel(),
+                                             ptr(out), stream_ptr()))
+
+
+def stat_kpp_commit(D, pot, closest, cand, centre) -> None:
+    N, ntr = D.shape
+    check(lib().atomai_b200_stat_kpp_commit(ptr(D), ntr, ptr(pot), ptr(closest), N, ptr(cand),
+                                            cand.shape[1], ptr(centre), stream_ptr()))
+
+
 def peak_refine(stack, atoms, dmax: int, popt, info, nfev=None) -> None:
     """One lmdif fit of a rotated 2-D Gaussian per int32 row (frame, row0, col0, d) of `atoms` to
     the windows of the fp32 (n, H, W) `stack`: popt (K, 7) float64, info / nfev (K,) int32."""

@@ -1,4 +1,4 @@
-from .coords import (find_com, get_lengthscale_constraints, get_nn_distances_, grid2xy,
+from .coords import (find_com, get_intensities, get_lengthscale_constraints, get_nn_distances_, grid2xy,
                      imcoordgrid, peak_refinement, remove_edge_coord, transform_coordinates)
 from .img import (crop_borders, cv_thresh, extract_random_subimages, extract_subimages,
                   extract_subimages_cuda, get_coord_grid,

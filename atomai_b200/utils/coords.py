@@ -216,3 +216,20 @@ def get_lengthscale_constraints(grid: np.ndarray) -> list:
     1 and half the largest index + 1 per dimension (atomai/utils/coords.py:540-543)."""
     upper = np.amax(grid, axis=0) // 2 + 1
     return [np.ones(grid.shape[-1]).tolist(), upper.tolist()]
+
+
+def get_intensities(coordinates_all: dict, nn_input: np.ndarray, r: int = 3) -> List[np.ndarray]:
+    """Mean intensity of the r x r square (rows and columns from x - r//2, odd r centred) around
+    the rounded (x, y) of every atom, one array per frame key of `coordinates_all`, with frame k
+    taken from nn_input[k] (atomai/utils/coords.py:234-275)."""
+    out = []
+    h = r // 2
+    hi = h + 1 if r % 2 else h
+    for k, coord in coordinates_all.items():
+        img = nn_input[k]
+        vals = []
+        for c in coord:
+            cx, cy = int(np.around(c[0])), int(np.around(c[1]))
+            vals.append(np.mean(img[cx - h:cx + hi, cy - h:cy + hi]))
+        out.append(np.array(vals))
+    return out

@@ -444,6 +444,53 @@ int atomai_b200_augment(const float* x, float* y, float* scratch, const int64_t*
                         int h, int w, float in_min, float in_max, uint64_t seed, float* minmax,
                         void* stream);
 
+/* ---- k-means and Gaussian-mixture EM over a sub-image stack (csrc/stat.cu) ---------------------
+ * X: N x d fp32 row-major; mu (d): the column mean, subtracted on every load (X is never copied);
+ * 1 <= K <= 64 components.  Row sums go through the ordered per-CTA slots: identical bits on repeat.
+ * estep: s_nk = sum_j A_kj x_nj (+ B_kj x_nj^2 in mode 0) on centred rows, then per mode
+ *   0 GMM:     l_nk = s_nk + cst_k; resp (N x K, nullable) = softmax_k l, labels (nullable) = argmax,
+ *              out[0] = sum_n logsumexp_k l_nk;
+ *   1 k-means: dist_nk = ||x_n||^2 + s_nk + cst_k; labels (in: previous labels, out: first argmin),
+ *              rowval (nullable) = min distance, out[0] = sum of min distances, *changes (nullable)
+ *              += number of rows whose label changed;
+ *   2 k-means++ candidates: D (N x K) = dist, out[k] = sum_n min(closest_n, D_nk).
+ * accum: sx (K x d) = sum_n r_nk x_n, sxx (K x d, nullable) = sum_n r_nk x_n^2, nk (K, nullable) =
+ *   sum_n r_nk (float64) with r = resp (N x K) if given, else one-hot labels if given, else r_n0 = 1
+ *   (mu may be NULL: raw X).
+ * gmm_params: sklearn's diag (spherical = 0) / spherical M-step from accum's sums of centred X:
+ *   nk + 10 eps, means, covs (K x d or K, + reg_covar), weights (nk / N if init, else normalised),
+ *   and the E-step operands A = means * prec, B = -prec / 2, cst = log N(0) constant + log weight.
+ * kmeans_centres: c_new = sx / nk (empty clusters keep c_old), *shift = sum ||c_new - c_old||^2;
+ *   sx == NULL: c_new holds the centres already.  Both form A = -2 c, cst = ||c||^2.
+ * kpp_candidates: ntr <= 32 indices drawn with hash_uniform(counter + t, seed): proportional to
+ *   closest (numpy searchsorted over its fixed-order prefix sum), uniform if closest == NULL;
+ *   chunk_ws: atomai_b200_stat_kpp_chunks(N) doubles.
+ * estep / accum `math` (AB_MATH_*): FP32 exact FFMA kernels; TF32 / TF32X3 the wgmma kernels
+ *   (TF32X3: split operands, three MMAs per product).
+ * gather_rows: out (n x d) = X[idx] - mu.  kpp_commit: best = first argmin of pot (ntr),
+ *   closest = min(closest, D[:, best]), centre (d) = cand[best]. */
+int atomai_b200_stat_estep(const float* X, const float* mu, int N, int d, int K, int mode,
+                           const float* A, const float* B, const float* cst, const float* closest,
+                           float* resp, int* labels, float* rowval, float* D, double* out,
+                           double* changes, int math, void* stream);
+int atomai_b200_stat_accum(const float* X, const float* mu, int N, int d, int K, const float* resp,
+                           const int* labels, double* sx, double* sxx, double* nk, int math,
+                           void* stream);
+int atomai_b200_stat_gmm_params(const double* sx, const double* sxx, const double* nk, int N, int d,
+                                int K, int spherical, double reg_covar, int init, float* means,
+                                float* covs, float* weights, float* A, float* B, float* cst,
+                                void* stream);
+int atomai_b200_stat_kmeans_centres(const double* sx, const double* nk, const float* c_old,
+                                    float* c_new, int K, int d, float* A, float* cst, double* shift,
+                                    void* stream);
+int64_t atomai_b200_stat_kpp_chunks(int N);
+int atomai_b200_stat_kpp_candidates(const float* closest, int N, int ntr, uint64_t seed,
+                                    uint64_t counter, double* chunk_ws, int* idx, void* stream);
+int atomai_b200_stat_gather_rows(const float* X, const float* mu, int d, const int* idx, int n,
+                                 float* out, void* stream);
+int atomai_b200_stat_kpp_commit(const float* D, int ntr, const double* pot, float* closest, int N,
+                                const float* cand, int d, float* centre, void* stream);
+
 /* ---- multi-GPU: small all-reduce over NVLink peer memory (csrc/p2p.cu) -----------------
  * Every rank exposes a zero-initialised mailbox (atomai_b200_p2p_data_bytes) and flag buffer
  * (atomai_b200_p2p_flag_bytes) to its peers (CUDA IPC: atomai_b200_ipc_export gives the 64-byte
