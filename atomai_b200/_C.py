@@ -16,7 +16,8 @@ LIB_PATH = os.path.join(_HERE, "libatomai_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
-           "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu"]
+           "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu",
+           "decomp.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -160,6 +161,12 @@ SIGNATURES = {
     "atomai_b200_stat_kpp_candidates": (_i, [_vp, _i, _i, C.c_uint64, C.c_uint64, _vp, _vp, _vp]),
     "atomai_b200_stat_gather_rows": (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp]),
     "atomai_b200_stat_kpp_commit": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp]),
+    "atomai_b200_decomp_slot_doubles": (_i64, [_i, _i, _i, _i]),
+    "atomai_b200_decomp_gram": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
+    "atomai_b200_decomp_project": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _i, _vp]),
+    "atomai_b200_decomp_nmf_w": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "atomai_b200_decomp_nmf_h": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "atomai_b200_decomp_ica_step": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
     "atomai_b200_prob_mask": (_i, [_vp, _i, _i64, _i, _i, _f, _vp, _i, _vp, _vp]),
     "atomai_b200_gather_windows": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
     "atomai_b200_peak_refine": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),

@@ -606,6 +606,69 @@ def stat_kpp_commit(D, pot, closest, cand, centre) -> None:
                                             cand.shape[1], ptr(centre), stream_ptr()))
 
 
+DECOMP_MAX_K = 64      # components per decomp_project call and limit of the NMF / FastICA passes
+
+
+def decomp_slot_doubles(op: int, N: int, d: int, K: int) -> int:
+    """ordered-slot workspace (doubles) of a decomp pass: op 0 / 1 gram (rows = op), 2 nmf_w,
+    3 nmf_h, 4 ica_step"""
+    return int(lib().atomai_b200_decomp_slot_doubles(op, N, d, K))
+
+
+def decomp_gram(X, mu, G, rows: bool) -> None:
+    """float64 G = (X - mu)^T (X - mu) (d x d), or (X - mu)(X - mu)^T (N x N) when `rows`; mu
+    (d,) fp32 or None.  Exact fp32 FFMA whatever set_math says."""
+    N, d = X.shape
+    m = N if rows else d
+    assert X.is_contiguous() and X.dtype == torch.float32
+    assert G.dtype == torch.float64 and G.shape == (m, m) and G.is_contiguous()
+    check(lib().atomai_b200_decomp_gram(ptr(X), ptr(mu), N, d, int(rows), ptr(G), stream_ptr()))
+
+
+def decomp_project(X, mu, B, out) -> None:
+    """fp32 out (N, k) = (X - mu) B^T for B (k, d), any k (blocks of DECOMP_MAX_K rows of B)."""
+    N, d = X.shape
+    k = B.shape[0]
+    assert X.is_contiguous() and X.dtype == B.dtype == out.dtype == torch.float32
+    assert B.shape == (k, d) and B.is_contiguous() and out.shape == (N, k) and out.is_contiguous()
+    for k0 in range(0, k, DECOMP_MAX_K):
+        kb = min(DECOMP_MAX_K, k - k0)
+        check(lib().atomai_b200_decomp_project(ptr(X), ptr(mu), N, d, kb, B[k0].data_ptr(),
+                                               out[:, k0].data_ptr(), k, stream_ptr()))
+
+
+def decomp_nmf_w(X, H, HHt, W, out) -> None:
+    """one coordinate-descent sweep of W (N, k) in place; out (k * k + 1,) float64 <- [W^T W,
+    violation]"""
+    N, d = X.shape
+    k = H.shape[0]
+    assert X.dtype == H.dtype == W.dtype == torch.float32 and HHt.dtype == out.dtype == torch.float64
+    assert W.shape == (N, k) and H.shape == (k, d) and HHt.shape == (k, k) and out.numel() == k * k + 1
+    assert all(t.is_contiguous() for t in (X, H, HHt, W, out))
+    check(lib().atomai_b200_decomp_nmf_w(ptr(X), N, d, k, ptr(H), ptr(HHt), ptr(W), ptr(out),
+                                         stream_ptr()))
+
+
+def decomp_nmf_h(WtX, WtW, H, out) -> None:
+    """one coordinate-descent sweep of H (k, d) in place from W^T X (k, d) and W^T W (float64);
+    out (k * k + 1,) float64 <- [H H^T, violation]"""
+    k, d = H.shape
+    assert H.dtype == torch.float32 and WtX.dtype == WtW.dtype == out.dtype == torch.float64
+    assert WtX.shape == (k, d) and WtW.shape == (k, k) and out.numel() == k * k + 1
+    assert all(t.is_contiguous() for t in (WtX, WtW, H, out))
+    check(lib().atomai_b200_decomp_nmf_h(ptr(WtX), ptr(WtW), d, k, ptr(H), ptr(out), stream_ptr()))
+
+
+def decomp_ica_step(X1, W, out) -> None:
+    """FastICA pass over the whitened samples X1 (N, k) fp32 with W (k, k) float64: out (k * k + k,)
+    float64 <- [sum_n tanh(W x_n) x_n^T, sum_n (1 - tanh(W x_n)^2)]"""
+    N, k = X1.shape
+    assert X1.dtype == torch.float32 and W.dtype == out.dtype == torch.float64
+    assert W.shape == (k, k) and out.numel() == k * k + k
+    assert all(t.is_contiguous() for t in (X1, W, out))
+    check(lib().atomai_b200_decomp_ica_step(ptr(X1), N, k, ptr(W), ptr(out), stream_ptr()))
+
+
 def peak_refine(stack, atoms, dmax: int, popt, info, nfev=None) -> None:
     """One lmdif fit of a rotated 2-D Gaussian per int32 row (frame, row0, col0, d) of `atoms` to
     the windows of the fp32 (n, H, W) `stack`: popt (K, 7) float64, info / nfev (K,) int32."""

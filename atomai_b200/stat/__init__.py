@@ -1,3 +1,4 @@
+from .decomposition import NMF, PCA, FastICA
 from .mixture import MAX_COMPONENTS, GaussianMixture, KMeans
 from .multivar import calculate_transition_matrix, imlocal, sum_transitions, update_classes
 
@@ -20,4 +21,5 @@ class SpectralUnmixer:
 
 
 __all__ = ['imlocal', 'calculate_transition_matrix', 'sum_transitions', 'update_classes',
-           'SlidingFFTNMF', 'SpectralUnmixer', 'GaussianMixture', 'KMeans', 'MAX_COMPONENTS']
+           'SlidingFFTNMF', 'SpectralUnmixer', 'GaussianMixture', 'KMeans', 'PCA', 'NMF', 'FastICA',
+           'MAX_COMPONENTS']

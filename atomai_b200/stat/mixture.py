@@ -61,10 +61,17 @@ def _device_matrix(X, K: int) -> torch.Tensor:
     N, d = _shape(X)
     if N < K:
         raise ValueError(f"n_samples={N} should be >= n_components={K}")
+    return _as_device(X, lambda copy: _check_memory(N, d, K, copy))
+
+
+def _as_device(X, check_memory) -> torch.Tensor:
+    """X as a contiguous fp32 (N, d) CUDA tensor (X itself when it already is one), after
+    check_memory(copy) has been told whether a copy of X is made."""
+    N, d = _shape(X)
     if not torch.cuda.is_available():
         raise RuntimeError("atomai_b200.stat needs a CUDA device (there is no CPU path)")
     host = not (isinstance(X, torch.Tensor) and X.is_cuda)
-    _check_memory(N, d, K, host or X.dtype != torch.float32 or not X.is_contiguous())
+    check_memory(host or X.dtype != torch.float32 or not X.is_contiguous())
     if host:
         X = torch.from_numpy(np.ascontiguousarray(np.asarray(X, dtype=np.float32)))
         return X.reshape(N, d).cuda()

@@ -491,6 +491,34 @@ int atomai_b200_stat_gather_rows(const float* X, const float* mu, int d, const i
 int atomai_b200_stat_kpp_commit(const float* D, int ntr, const double* pot, float* closest, int N,
                                 const float* cand, int d, float* centre, void* stream);
 
+/* ---- PCA / NMF / FastICA passes over a sub-image stack (csrc/decomp.cu) ----------------------
+ * X: N x d fp32 row-major, read in place; mu (d, nullable): subtracted on every load.  Exact fp32
+ * FFMA for the contractions over X, float64 for everything else; the set_math mode does not apply.
+ * Row sums go through the ordered per-CTA slots: identical bits on repeat.  1 <= K <= 64.
+ * gram: rows = 0: G (d x d) = (X - mu)^T (X - mu); rows = 1: G (N x N) = (X - mu)(X - mu)^T;
+ *   float64, exactly symmetric (upper-triangle tiles, mirrored).
+ * project: out[n * ldo + k] = sum_j (X_nj - mu_j) B_kj for the K rows of B (K x d fp32).
+ * nmf_w: one coordinate-descent sweep (sklearn's _update_cdnmf_fast, Frobenius, no regularisation)
+ *   of W (N x K fp32, in place) against H (K x d fp32) and HHt (K x K float64), with XHt = X H^T
+ *   formed per row tile; out (K * K + 1 doubles) = [W^T W of the updated W, violation].
+ * nmf_h: the same sweep of H (K x d, in place) from WtX (K x d float64, sum_n W_nk X_n:
+ *   atomai_b200_stat_accum with resp = W, mu = NULL) and WtW (K x K); out = [H H^T, violation].
+ * ica_step: X1 (N x K fp32 row-major: the whitened samples), W (K x K float64); with
+ *   g = tanh(W x1) per sample, out (K * K + K doubles) = [sum_n g x1^T, sum_n (1 - g^2)].
+ * slot_doubles: the ordered-slot workspace (doubles) a call takes, op 0/1 gram (rows = op),
+ *   2 nmf_w, 3 nmf_h, 4 ica_step; -1 for bad arguments. */
+int64_t atomai_b200_decomp_slot_doubles(int op, int N, int d, int K);
+int atomai_b200_decomp_gram(const float* X, const float* mu, int N, int d, int rows, double* G,
+                            void* stream);
+int atomai_b200_decomp_project(const float* X, const float* mu, int N, int d, int K, const float* B,
+                               float* out, int ldo, void* stream);
+int atomai_b200_decomp_nmf_w(const float* X, int N, int d, int K, const float* H, const double* HHt,
+                             float* W, double* out, void* stream);
+int atomai_b200_decomp_nmf_h(const double* WtX, const double* WtW, int d, int K, float* H,
+                             double* out, void* stream);
+int atomai_b200_decomp_ica_step(const float* X1, int N, int K, const double* W, double* out,
+                                void* stream);
+
 /* ---- multi-GPU: small all-reduce over NVLink peer memory (csrc/p2p.cu) -----------------
  * Every rank exposes a zero-initialised mailbox (atomai_b200_p2p_data_bytes) and flag buffer
  * (atomai_b200_p2p_flag_bytes) to its peers (CUDA IPC: atomai_b200_ipc_export gives the 64-byte
