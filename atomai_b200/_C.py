@@ -17,7 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
            "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu",
-           "decomp.cu"]
+           "decomp.cu", "ed_ops.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -108,6 +108,9 @@ SIGNATURES = {
     "atomai_b200_resize_bwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "atomai_b200_upsample2x_fwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "atomai_b200_upsample2x_bwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "atomai_b200_avgpool_fwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "atomai_b200_upsample_w2x_fwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp]),
+    "atomai_b200_upsample_w2x_bwd": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp]),
     "atomai_b200_conv3x3_fwd": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i,
                                      _i, _vp, _vp]),
     "atomai_b200_conv3x3_wgrad": (_i, [_vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i,

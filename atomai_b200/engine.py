@@ -398,6 +398,33 @@ class Tape:
             return self.materialize(Act(x.t, x.scale, x.shift, parent=x, needs_grad=x.needs_grad, up=mode))
         return Act(x.t, x.scale, x.shift, parent=x, needs_grad=x.needs_grad, up=mode)
 
+    def upsample_w2x(self, x: Act) -> Act:
+        """F.interpolate(scale_factor=2, mode="nearest") of a 1-D signal stored as (N, 1, w, C):
+        the width doubles, the unit height stays (ImSpec's 1-D decoder_upsampling,
+        atomai/nets/ed.py:151-154).  `upsample` cannot serve: a 2-D map whose height is 1 still
+        doubles along both axes."""
+        x = self.materialize(x)
+        n, h, w, c = x.t.shape
+        assert h == 1, f"upsample_w2x expects a (N, 1, w, C) signal, got {tuple(x.t.shape)}"
+        out_t = torch.empty((n, 1, 2 * w, c), device=x.t.device, dtype=torch.float32)
+        ops.upsample_w2x_fwd(x.t, out_t)
+        out = Act(out_t, needs_grad=x.needs_grad)
+        if self.record:
+            self.ops.append(("custom", _UpW2xRec(x, out)))
+        return out
+
+    def avgpool(self, x: Act, sh: int, sw: int) -> Act:
+        """F.avg_pool2d(x, (sh, sw)) with floor semantics (ImSpec's encoder_downsampling,
+        atomai/nets/ed.py:70-76).  Forward only: it pools the network input."""
+        if x.needs_grad:
+            raise NotImplementedError("avgpool has no backward: its input must not require a gradient")
+        if x.pending():
+            x = self.materialize(x)
+        n, h, w, c = x.t.shape
+        out_t = torch.empty((n, h // sh, w // sw, c), device=x.t.device, dtype=torch.float32)
+        ops.avgpool_fwd(x.t, out_t, sh, sw)
+        return Act(out_t, needs_grad=False)
+
     @staticmethod
     def _up_grad(s: Act, g: torch.Tensor) -> None:
         """parent.grad (+)= upsample^T(g) (g: gradient w.r.t. the upsampled, affine'd values)."""
@@ -874,6 +901,20 @@ class _ResizeRec:
             return
         dx = torch.zeros(self.x.t.shape, device=g.device, dtype=torch.float32)
         ops.resize_bwd(_dense(g), dx, self.factor, self.bilinear)
+        _acc_grad(self.x, dx, True)
+
+
+class _UpW2xRec:
+    def __init__(self, x, out):
+        self.x, self.out = x, out
+
+    def backward(self, tape):
+        g = self.out.grad
+        self.out.grad = None
+        if g is None or not self.x.needs_grad:
+            return
+        dx = torch.empty(self.x.t.shape, device=g.device, dtype=torch.float32)
+        ops.upsample_w2x_bwd(g, dx)
         _acc_grad(self.x, dx, True)
 
 

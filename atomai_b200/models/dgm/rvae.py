@@ -43,10 +43,10 @@ class rVAE(BaseVAE):
     def forward_compute_elbo(self, x: torch.Tensor, y: Optional[torch.Tensor] = None,
                              mode: str = "train", eps: Optional[torch.Tensor] = None
                              ) -> torch.Tensor:
-        """rVAE forward pass with ELBO (rvae.py:110-147).  `eps` (optional) fixes the
-        reparameterisation noise (tests)."""
-        if y is not None:
-            raise NotImplementedError("class-conditioned rVAE is outside the native hot path")
+        """rVAE forward pass with ELBO (rvae.py:110-147).  `y` (int64 labels, validated by fit)
+        appends the one-hot class vector to the content latents the spatial decoder sees.  `eps`
+        (optional) fixes the reparameterisation noise (tests)."""
+        self._require_labels(y)
         grad = mode != "eval"
         with torch.set_grad_enabled(grad):
             z_mean, z_logsd = self.encoder_net(x)
@@ -60,13 +60,17 @@ class rVAE(BaseVAE):
                 zc = z[:, 3:]
             else:
                 dx, zc = None, z[:, 1:]
+            if y is not None:
+                zc = torch.cat((zc, self._onehot(y)), -1)
             x_reconstr = self.decoder_net.decode(zc, phi, dx)
             return self.elbo_fn(x, x_reconstr, z_mean, z_logsd, **self.kdict_)
 
     def fit(self, X_train, y_train=None, X_test=None, y_test=None, loss: str = "mse", **kwargs):
         """Trains rVAE model (rvae.py:149-215): kwargs rotation_prior, translation_prior,
-        capacity, training_cycles, batch_size, filename."""
+        capacity, training_cycles, batch_size, filename.  With nb_classes > 0, y_train (and y_test
+        with X_test) are the class labels 0 .. nb_classes - 1 of the class-conditioned rVAE."""
         self._check_inputs(X_train, y_train, X_test, y_test)
+        y_train, y_test = self._check_labels(X_test, y_train, y_test)
         self.dx_prior = kwargs.get("translation_prior", 0.1)
         self.kdict_["phi_prior"] = kwargs.get("rotation_prior", 0.1)
         for k, v in kwargs.items():

@@ -16,6 +16,31 @@ from ...utils.coords import imcoordgrid
 from ...utils.nn import set_train_rng
 
 
+def _host(y) -> np.ndarray:
+    if isinstance(y, torch.Tensor):
+        return y.detach().cpu().numpy()
+    return np.asarray(y)
+
+
+def host_labels(y, nb_classes: int) -> np.ndarray:
+    """Class labels (int, array-like or tensor) as a 1-d int64 host array, checked against
+    nb_classes the way the reference's to_onehot does (atomai/utils/preproc.py:916-923), and
+    additionally refused when negative or not integral."""
+    y = _host(y).reshape(-1)
+    if y.dtype == np.bool_ or not (np.issubdtype(y.dtype, np.integer)
+                                   or np.issubdtype(y.dtype, np.floating)):
+        raise ValueError(f"class labels must be integers, got dtype {y.dtype}")
+    if y.size and y.max() >= nb_classes:
+        raise AssertionError(
+            "Labelling must start from 0 and "
+            "maximum label value must be less than total number of classes")
+    if np.issubdtype(y.dtype, np.floating) and not np.all(np.floor(y) == y):
+        raise ValueError("class labels must be integers, got non-integral values")
+    if y.size and y.min() < 0:
+        raise ValueError(f"class labels must be non-negative, got {y.min()}")
+    return y.astype(np.int64)
+
+
 class BaseVAE(viBaseTrainer):
     """
     General class for VAE models (atomai/models/dgm/vae.py:28-103).
@@ -133,13 +158,27 @@ class BaseVAE(viBaseTrainer):
             imgdata_.append(img_)
         return np.array(imgdata_), np.array(imgdata_encoded)
 
-    def decode(self, z_sample: Union[np.ndarray, torch.Tensor], y=None) -> np.ndarray:
+    def decode(self, z_sample: Union[np.ndarray, torch.Tensor],
+               y: Optional[Union[int, np.ndarray, torch.Tensor]] = None) -> np.ndarray:
         """Decodes latent vector(s) into images (vae.py:178-221).  For coord > 0 the decoder is
-        evaluated on the untransformed pixel grid, as in the reference."""
+        evaluated on the untransformed pixel grid, as in the reference.  A class-conditioned model
+        needs `y`: an int, a 0-d / 1-d array or a tensor of labels; a single label applies to
+        every row of z_sample."""
         if isinstance(z_sample, np.ndarray):
             z_sample = torch.from_numpy(z_sample).float()
         if z_sample.ndim == 1:
             z_sample = z_sample[None]
+        if y is not None or self.nb_classes:
+            if y is None:
+                raise ValueError(f"this model is class-conditioned (nb_classes={self.nb_classes}): "
+                                 "pass the label(s) y to decode")
+            labels = host_labels(y, self.nb_classes)
+            if labels.size == 1:
+                labels = np.broadcast_to(labels.reshape(1), (len(z_sample),))
+            elif len(labels) != len(z_sample):
+                raise ValueError(f"got {len(labels)} labels for {len(z_sample)} latent vectors")
+            onehot = torch.from_numpy(np.eye(self.nb_classes, dtype=np.float32)[labels])
+            z_sample = torch.cat([z_sample.float().cpu(), onehot], 1)
         z_sample = z_sample.to(self.device)
         self.decoder_net.eval()
         with torch.no_grad():
@@ -152,13 +191,21 @@ class BaseVAE(viBaseTrainer):
         return x_decoded.cpu().numpy()
 
     def reconstruct(self, x_new, **kwargs: int) -> np.ndarray:
-        """encode -> decode of the latent mean (vae.py:223-271).  The joint VAEs append the encoded
-        alphas, or with `label` (an int, or one int per discrete head) the one-hot class vector."""
+        """encode -> decode of the latent mean (vae.py:223-271).  A class-conditioned model needs
+        `label` (one label for every row, or one per row) and decodes with its one-hot appended.
+        The joint VAEs append the encoded alphas, or with `label` (an int, or one int per discrete
+        head) the one-hot class vector."""
         if not self.discrete_dim:
+            label = kwargs.get("label")
+            if self.nb_classes and label is None:
+                raise ValueError(f"this model is class-conditioned (nb_classes={self.nb_classes}): "
+                                 "pass label=... to reconstruct")
+            if label is not None:
+                host_labels(label, self.nb_classes)
             z_mean, _ = self.encode(x_new, **kwargs)
             if self.coord > 0:
                 z_mean = z_mean[:, self.coord:]
-            return self.decode(z_mean)
+            return self.decode(z_mean, label)
         z_mean, _, alphas = self.encode(x_new, **kwargs)
         z_mean = z_mean[:, self.coord:]
         label = kwargs.get("label")
@@ -177,6 +224,50 @@ class BaseVAE(viBaseTrainer):
             raise RuntimeError("Training data must have the same dimensions as in_dim")
         if X_test is not None and tuple(X_test.shape[1:]) != tuple(X_train.shape[1:]):
             raise RuntimeError("Test data must have the same dimensions as the training data")
+        if y_train is not None and self.nb_classes == 0:
+            raise RuntimeError(
+                "You must have forgotten to specify number of classes " +
+                "during the initialization. Example of correct usage: " +
+                "vae = VAE(in_dim=(28, 28), nb_classes=10)); " +
+                "vae.fit(train_data, train_labels).")
+        lbl_match = True
+        if y_train is not None and y_test is None:
+            lbl_match = self.nb_classes == len(np.unique(_host(y_train)))
+        elif y_train is not None and y_test is not None:
+            lbl_match = (self.nb_classes == len(np.unique(_host(y_train)))
+                         == len(np.unique(_host(y_test))))
+        if not lbl_match:
+            raise RuntimeError(
+                "The number of classes specified at initialization must be " +
+                "equal the the number of classes in train and test labels")
+
+    def _check_labels(self, X_test, y_train, y_test):
+        """Labels of a class-conditioned fit, validated on the host and cast to int64 before any
+        device work (the reference scatters them on the device: a negative or fractional label
+        fails there, a missing one fails inside the decoder)."""
+        if self.nb_classes:
+            if y_train is None:
+                raise ValueError(f"this model is class-conditioned (nb_classes={self.nb_classes}): "
+                                 "pass the training labels y_train to fit")
+            if X_test is not None and y_test is None:
+                raise ValueError(f"this model is class-conditioned (nb_classes={self.nb_classes}): "
+                                 "pass the test labels y_test with X_test")
+        if y_train is not None:
+            y_train = torch.from_numpy(host_labels(y_train, self.nb_classes))
+        if y_test is not None:
+            y_test = torch.from_numpy(host_labels(y_test, self.nb_classes))
+        return y_train, y_test
+
+    def _require_labels(self, y) -> None:
+        if y is not None and not self.nb_classes:
+            raise RuntimeError("labels were passed to a model built with nb_classes=0")
+        if y is None and self.nb_classes:
+            raise ValueError(f"this model is class-conditioned (nb_classes={self.nb_classes}): "
+                             "its forward pass needs the labels y")
+
+    def _onehot(self, y: torch.Tensor) -> torch.Tensor:
+        """(B,) int64 labels (already validated) -> (B, nb_classes) float one-hot, on y's device."""
+        return torch.zeros(len(y), self.nb_classes, device=y.device).scatter_(1, y.view(-1, 1), 1.0)
 
     def update_metadict(self):
         self.metadict["num_epochs"] = self.current_epoch
@@ -217,10 +308,10 @@ class VAE(BaseVAE):
     def forward_compute_elbo(self, x: torch.Tensor, y: Optional[torch.Tensor] = None,
                              mode: str = "train", eps: Optional[torch.Tensor] = None
                              ) -> torch.Tensor:
-        """VAE forward pass with ELBO (vae.py:661-687).  `eps` (optional) fixes the
+        """VAE forward pass with ELBO (vae.py:661-687).  `y` (int64 labels, validated by fit)
+        appends the one-hot class vector to the decoder input.  `eps` (optional) fixes the
         reparameterisation noise (tests)."""
-        if y is not None:
-            raise NotImplementedError("class-conditioned VAE is outside the native hot path")
+        self._require_labels(y)
         grad = mode != "eval"
         with torch.set_grad_enabled(grad):
             z_mean, z_logsd = self.encoder_net(x)
@@ -228,13 +319,17 @@ class VAE(BaseVAE):
                 self.kdict_["num_iter"] += 1
             z_sd = torch.exp(z_logsd)
             z = z_mean + z_sd * eps if eps is not None else self.reparameterize(z_mean, z_sd)
+            if y is not None:
+                z = torch.cat((z, self._onehot(y)), -1)
             x_reconstr = self.decoder_net(z)
             return self.elbo_fn(x, x_reconstr, z_mean, z_logsd, **self.kdict_)
 
     def fit(self, X_train, y_train=None, X_test=None, y_test=None, loss: str = "mse", **kwargs):
         """Trains VAE model (vae.py:689-743): kwargs capacity, training_cycles, batch_size,
-        filename."""
+        filename.  With nb_classes > 0, y_train (and y_test with X_test) are the class labels
+        0 .. nb_classes - 1 of the class-conditioned VAE."""
         self._check_inputs(X_train, y_train, X_test, y_test)
+        y_train, y_test = self._check_labels(X_test, y_train, y_test)
         for k, v in kwargs.items():
             if k in ["capacity"]:
                 self.kdict_[k] = v

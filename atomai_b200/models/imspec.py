@@ -31,6 +31,7 @@ class ImSpec(ImSpecTrainer):
             batch_size: int = 64, compute_accuracy: bool = False, full_epoch: bool = False,
             swa: bool = False, perturb_weights: bool = False, **kwargs):
         """Compiles a trainer and performs model training (imspec.py:63-145)."""
+        self._check_upsampling()
         self.compile_trainer((X_train, y_train, X_test, y_test), loss, optimizer, training_cycles,
                              batch_size, compute_accuracy, full_epoch, swa, perturb_weights,
                              **kwargs)
@@ -38,6 +39,7 @@ class ImSpec(ImSpecTrainer):
 
     def predict(self, data: np.ndarray, **kwargs) -> np.ndarray:
         """Apply the (trained) model to new data (imspec.py:147-163): returns (n, *out_dim)."""
+        self._check_upsampling()
         norm = kwargs.get("norm", False)
         if len(self.in_dim) == 2:
             x = torch_format_image(data, norm)
@@ -52,3 +54,11 @@ class ImSpec(ImSpecTrainer):
                 outs.append(self.net(x[i:i + bs].to(self.device)).cpu())
         out = torch.cat(outs).numpy()
         return out[:, 0] if out.shape[1] == 1 else out
+
+    def _check_upsampling(self) -> None:
+        """The 1-D decoder_upsampling path starts from length // 4 and doubles twice, so it can only
+        produce lengths that are multiples of 4 (the reference fails at the first loss otherwise)."""
+        if self.meta_state_dict.get("decoder_upsampling") and len(self.out_dim) == 1 \
+                and self.out_dim[0] % 4:
+            raise ValueError(f"decoder_upsampling=True needs a spectrum length that is a multiple "
+                             f"of 4, got out_dim={tuple(self.out_dim)}")

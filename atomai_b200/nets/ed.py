@@ -53,10 +53,12 @@ class SignalEncoder(nn.Module):
         self.reshape_ = nb_filters * n
         self.conv = ConvBlock(ndim, nb_layers, 1, nb_filters, lrelu_a=0.1, batch_norm=bn)
         self.fc = nn.Linear(nb_filters * n, z_dim)
+        self._ndim = ndim
 
     def _emit(self, tape: Tape, x: Act) -> Act:
-        if self.downsample:
-            raise NotImplementedError("encoder_downsampling (avg_pool) is not on the native path")
+        if self.downsample:         # avg_pool2d(x, s, s) / avg_pool1d on the (N, 1, L, 1) spectrum
+            s = self.downsample
+            x = tape.avgpool(x, s if self._ndim == 2 else 1, s)
         return tape.linear(tape.flatten(self.conv._emit(tape, x)), self.fc)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
@@ -102,10 +104,9 @@ class SignalDecoder(nn.Module):
         h, w = (self.reshape_[1], self.reshape_[2]) if self._ndim == 2 else (1, self.reshape_[1])
         x = tape.unflatten(tape.linear(z, self.fc), c, h, w)
         if self.upsampling:
-            if self._ndim != 2:
-                raise NotImplementedError("1-D decoder_upsampling is not on the native path")
-            x = tape.upsample(self.deconv1._emit(tape, x), "nearest")
-            x = tape.upsample(self.deconv2._emit(tape, x), "nearest")
+            up = (lambda a: tape.upsample(a, "nearest")) if self._ndim == 2 else tape.upsample_w2x
+            x = up(self.deconv1._emit(tape, x))
+            x = up(self.deconv2._emit(tape, x))
         x = self.dilblock._emit(tape, x)
         x = self.conv._emit(tape, x)
         return tape.conv(x, self.out, None, 1.0)

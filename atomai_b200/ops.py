@@ -203,6 +203,26 @@ def upsample_bwd(dy, dx, bilinear=True) -> None:
                                            1 if bilinear else 0, stream_ptr()))
 
 
+def avgpool_fwd(x, out, sh: int, sw: int) -> None:
+    """out (N, H//sh, W//sw, C) = sh x sw window averages of x (N, H, W, C)."""
+    N, H, W, Cc = x.shape
+    check(lib().atomai_b200_avgpool_fwd(ptr(x), _ld(x), ptr(out), _ld(out), N, H, W, Cc, int(sh),
+                                        int(sw), stream_ptr()))
+
+
+def upsample_w2x_fwd(x, out) -> None:
+    """Nearest x2 along the width of a (N, 1, w, C) signal."""
+    N, _, w, Cc = x.shape
+    check(lib().atomai_b200_upsample_w2x_fwd(ptr(x), _ld(x), ptr(out), _ld(out), N, w, Cc,
+                                             stream_ptr()))
+
+
+def upsample_w2x_bwd(dy, dx) -> None:
+    N, _, w, Cc = dx.shape
+    check(lib().atomai_b200_upsample_w2x_bwd(ptr(dy), _ld(dy), ptr(dx), _ld(dx), N, w, Cc,
+                                             stream_ptr()))
+
+
 def affine_res_act(a, scale, shift, res, slope, out) -> None:
     """out = LeakyReLU(a*scale + shift + res) (scale/shift/res optional)."""
     N, H, W, Cc = a.shape

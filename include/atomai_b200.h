@@ -163,6 +163,17 @@ int atomai_b200_upsample2x_fwd(const float* x, int ld_x, float* y, int ld_y, int
                                int C, int bilinear, void* stream);
 int atomai_b200_upsample2x_bwd(const float* dy, int ld_dy, float* dx, int ld_dx, int N, int h,
                                int w, int C, int bilinear, void* stream);
+/* ImSpec encoder_downsampling (atomai/nets/ed.py:66-79): y (N, H/sh, W/sw, C) = average over each
+ * sh x sw window of x (N, H, W, C), floor semantics; sum in row-major order times 1/(sh*sw).
+ * Images use (s, s), spectra stored as (N, 1, L, 1) use (1, s).  Forward only. */
+int atomai_b200_avgpool_fwd(const float* x, int ld_x, float* y, int ld_y, int N, int H, int W, int C,
+                            int sh, int sw, void* stream);
+/* 1-D decoder_upsampling (atomai/nets/ed.py:151-154): nearest x2 along the width of (N, 1, w, C)
+ * -> (N, 1, 2w, C), and its adjoint dx[i] = dy[2i] + dy[2i+1]. */
+int atomai_b200_upsample_w2x_fwd(const float* x, int ld_x, float* y, int ld_y, int N, int w, int C,
+                                 void* stream);
+int atomai_b200_upsample_w2x_bwd(const float* dy, int ld_dy, float* dx, int ld_dx, int N, int w, int C,
+                                 void* stream);
 /* ResBlock tail (atomai/nets/blocks.py:199-214): y = LeakyReLU(a*scale + shift + res) in one
  * pass; scale/shift (the BatchNorm affine) and res (the residual) may be NULL.  Backward mask:
  * g = dy * LeakyReLU'(y), read from sign(y) (slope > 0). */
