@@ -17,7 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
            "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu",
-           "decomp.cu", "ed_ops.cu"]
+           "decomp.cu", "ed_ops.cu", "graph.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -33,6 +33,7 @@ JLAT_MAX_CONT = 32       # AB_JLAT_MAX_CONT
 JLAT_MAX_DISC = 64       # AB_JLAT_MAX_DISC
 JLAT_ALPHAS = 0
 JLAT_SAMPLE = 1
+GRAPH_MAX_RING = 32     # AB_GRAPH_MAX_RING
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -170,6 +171,12 @@ SIGNATURES = {
     "atomai_b200_decomp_nmf_w": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "atomai_b200_decomp_nmf_h": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
     "atomai_b200_decomp_ica_step": (_i, [_vp, _i, _i, _vp, _vp, _vp]),
+    "atomai_b200_graph_cell_keys": (_i, [_vp, _vp, _i, C.POINTER(_d), _d, C.POINTER(_i64), _vp, _vp]),
+    "atomai_b200_graph_bonds": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i, C.POINTER(_d), _d,
+                                     C.POINTER(_i64), _vp, _vp, _vp]),
+    "atomai_b200_graph_hops": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "atomai_b200_graph_rings": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "atomai_b200_graph_ring_filter": (_i, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "atomai_b200_prob_mask": (_i, [_vp, _i, _i64, _i, _i, _f, _vp, _i, _vp, _vp]),
     "atomai_b200_gather_windows": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
     "atomai_b200_peak_refine": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),

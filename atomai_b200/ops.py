@@ -689,6 +689,82 @@ def decomp_ica_step(X1, W, out) -> None:
     check(lib().atomai_b200_decomp_ica_step(ptr(X1), N, k, ptr(W), ptr(out), stream_ptr()))
 
 
+def _grid_args(lo, dims):
+    return (C.c_double * 3)(*[float(v) for v in lo]), (C.c_int64 * 3)(*[int(v) for v in dims])
+
+
+def graph_cell_keys(pos, frame, lo, side: float, dims, keys) -> None:
+    """int64 cell key of every atom of pos (N, 3) float64: ((frame * nz + cz) * ny + cy) * nx + cx
+    for cells of side `side` from the origin lo (3 floats), dims = (nx, ny, nz); frame (N,) int32
+    or None."""
+    N = pos.shape[0]
+    assert pos.dtype == torch.float64 and pos.shape == (N, 3) and pos.is_contiguous()
+    assert keys.dtype == torch.int64 and keys.shape == (N,)
+    assert frame is None or (frame.dtype == torch.int32 and frame.shape == (N,))
+    lo_, dims_ = _grid_args(lo, dims)
+    check(lib().atomai_b200_graph_cell_keys(ptr(pos), ptr(frame), N, lo_, float(side), dims_,
+                                            ptr(keys), stream_ptr()))
+
+
+def graph_bonds(pos, cls, frame, keys, perm, cut, lo, side: float, dims, rowptr, out) -> None:
+    """Bonds within the C x C float64 cutoff table `cut` (class pair of cls, (N,) int32 or None).
+    keys / perm: the sorted cell keys and the atom of each.  rowptr None: out (N,) int32 = degrees;
+    else out[rowptr[i]:rowptr[i + 1]] = the atoms bonded to i, ascending."""
+    N = pos.shape[0]
+    Cn = cut.shape[0]
+    assert pos.dtype == cut.dtype == torch.float64 and pos.shape == (N, 3) and pos.is_contiguous()
+    assert cut.shape == (Cn, Cn) and cut.is_contiguous()
+    assert keys.dtype == perm.dtype == torch.int64 and keys.shape == perm.shape == (N,)
+    assert cls is None or (cls.dtype == torch.int32 and cls.shape == (N,))
+    assert frame is None or (frame.dtype == torch.int32 and frame.shape == (N,))
+    assert out.dtype == torch.int32 and (rowptr is not None or out.shape == (N,))
+    assert rowptr is None or (rowptr.dtype == torch.int64 and rowptr.shape == (N + 1,))
+    lo_, dims_ = _grid_args(lo, dims)
+    check(lib().atomai_b200_graph_bonds(ptr(pos), ptr(cls), ptr(frame), N, ptr(keys), ptr(perm),
+                                        ptr(cut), Cn, lo_, float(side), dims_, ptr(rowptr),
+                                        ptr(out), stream_ptr()))
+
+
+def graph_hops(rowptr, cols, bptr, ball, optr, out, cnt) -> None:
+    """One level of the packed (id << 5 | hops) hop table: optr None: cnt (N,) int64 = row lengths
+    of the next level; else out[optr[u]:optr[u + 1]] = u's next-level row."""
+    N = rowptr.shape[0] - 1
+    assert rowptr.dtype == bptr.dtype == torch.int64 and bptr.shape == (N + 1,)
+    assert cols.dtype == torch.int32 and ball.dtype == torch.int32
+    assert optr is None or (out is not None and out.dtype == torch.int32 and optr.shape == (N + 1,))
+    assert optr is not None or (cnt.dtype == torch.int64 and cnt.shape == (N,))
+    check(lib().atomai_b200_graph_hops(ptr(rowptr), ptr(cols), N, ptr(bptr), ptr(ball), ptr(optr),
+                                       ptr(out), ptr(cnt), stream_ptr()))
+
+
+def graph_rings(rowptr, cols, bptr, ball, max_depth: int, ring_base=None, atom_base=None,
+                lens=None, atoms=None, cnt=None) -> None:
+    """Rings of 3 ... max_depth atoms, one search per root atom.  ring_base None: cnt (N, 3) int64
+    = (rings, ring atoms, search steps) per root; else the rings of root r go to
+    lens[ring_base[r]:] and atoms[atom_base[r]:] (int32) in discovery order."""
+    N = rowptr.shape[0] - 1
+    assert rowptr.dtype == bptr.dtype == torch.int64 and bptr.shape == (N + 1,)
+    assert cols.dtype == torch.int32 and ball.dtype == torch.int32
+    if ring_base is None:
+        assert cnt.dtype == torch.int64 and cnt.shape == (N, 3) and cnt.is_contiguous()
+    else:
+        assert ring_base.dtype == atom_base.dtype == torch.int64 and ring_base.shape == (N,)
+        assert lens.dtype == atoms.dtype == torch.int32
+    check(lib().atomai_b200_graph_rings(ptr(rowptr), ptr(cols), N, ptr(bptr), ptr(ball),
+                                        int(max_depth), ptr(ring_base), ptr(atom_base), ptr(lens),
+                                        ptr(atoms), ptr(cnt), stream_ptr()))
+
+
+def graph_ring_filter(off, lens, atoms, bptr, ball, keep) -> None:
+    """keep (R,) uint8: 0 for the rings with a shortcut through the bond graph, else 1."""
+    R = lens.shape[0]
+    assert off.dtype == bptr.dtype == torch.int64 and off.shape == (R,)
+    assert lens.dtype == atoms.dtype == ball.dtype == torch.int32
+    assert keep.dtype == torch.uint8 and keep.shape == (R,)
+    check(lib().atomai_b200_graph_ring_filter(ptr(off), ptr(lens), ptr(atoms), R, ptr(bptr),
+                                              ptr(ball), ptr(keep), stream_ptr()))
+
+
 def peak_refine(stack, atoms, dmax: int, popt, info, nfev=None) -> None:
     """One lmdif fit of a rotated 2-D Gaussian per int32 row (frame, row0, col0, d) of `atoms` to
     the windows of the fp32 (n, H, W) `stack`: popt (K, 7) float64, info / nfev (K,) int32."""

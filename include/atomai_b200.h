@@ -530,6 +530,42 @@ int atomai_b200_decomp_nmf_h(const double* WtX, const double* WtW, int d, int K,
 int atomai_b200_decomp_ica_step(const float* X1, int N, int K, const double* W, double* out,
                                 void* stream);
 
+/* ---- bond graphs and rings of atomic lattices (csrc/graph.cu) --------------------------------
+ * pos: N x 3 float64 (Å); cls (N int32, nullable = all 0) indexes the C x C float64 cutoff table
+ * `cut`; frame (N int32, nullable = all 0) keeps the frames of a batch apart.  Grid: cell side
+ * `side` (>= every cutoff), origin lo_host[3] and dims_host[3] cells (HOST arrays).
+ * cell_keys: keys[i] = ((frame * nz + cz) * ny + cy) * nx + cx; the caller sorts them stably
+ *   (keys ascending, perm = the atom of each sorted key, int64).
+ * bonds: rowptr == NULL: out[i] = degree of i; else out[rowptr[i] ...] = the atoms bonded to i,
+ *   ascending.  Bonded: i != j and |p_i - p_j| <= cut[cls_i * C + cls_j].
+ * hops: one level of the hop table.  Rows bptr/ball hold packed words (id << 5 | hops), sorted;
+ *   level 0 is {u << 5} per atom.  optr == NULL: cnt[u] = length of u's next-level row (the union of
+ *   u's row and its bonded atoms' rows + 1 hop, least hops per id); else out[optr[u] ...] = that
+ *   row.  N < 2^26.
+ * rings: the hop table of radius max_depth / 2 in bptr/ball; 3 <= max_depth <= AB_GRAPH_MAX_RING.
+ *   ring_base == NULL: cnt[3 r ...] = (rings, their atoms, search steps) of root r; else root r's
+ *   rings in discovery order go to lens[ring_base[r] ...] and atoms[atom_base[r] ...].
+ * ring_filter: keep[r] = 0 when two atoms j < k of ring r (atoms[off[r] ...], lens[r] atoms) are
+ *   fewer than min(k - j, lens[r] - k + j) hops apart, else 1. */
+#define AB_GRAPH_MAX_RING 32
+int atomai_b200_graph_cell_keys(const double* pos, const int* frame, int N, const double* lo_host,
+                                double side, const int64_t* dims_host, int64_t* keys,
+                                void* stream);
+int atomai_b200_graph_bonds(const double* pos, const int* cls, const int* frame, int N,
+                            const int64_t* keys, const int64_t* perm, const double* cut, int C,
+                            const double* lo_host, double side, const int64_t* dims_host,
+                            const int64_t* rowptr, int* out, void* stream);
+int atomai_b200_graph_hops(const int64_t* rowptr, const int* cols, int N, const int64_t* bptr,
+                           const uint32_t* ball, const int64_t* optr, uint32_t* out, int64_t* cnt,
+                           void* stream);
+int atomai_b200_graph_rings(const int64_t* rowptr, const int* cols, int N, const int64_t* bptr,
+                            const uint32_t* ball, int max_depth, const int64_t* ring_base,
+                            const int64_t* atom_base, int* lens, int* atoms, int64_t* cnt,
+                            void* stream);
+int atomai_b200_graph_ring_filter(const int64_t* off, const int* lens, const int* atoms,
+                                  int64_t R, const int64_t* bptr, const uint32_t* ball,
+                                  unsigned char* keep, void* stream);
+
 /* ---- multi-GPU: small all-reduce over NVLink peer memory (csrc/p2p.cu) -----------------
  * Every rank exposes a zero-initialised mailbox (atomai_b200_p2p_data_bytes) and flag buffer
  * (atomai_b200_p2p_flag_bytes) to its peers (CUDA IPC: atomai_b200_ipc_export gives the 64-byte
