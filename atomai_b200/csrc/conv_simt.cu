@@ -671,11 +671,6 @@ __global__ void __launch_bounds__(256) conv_pix_quad_kernel(const ConvSimtParams
   }
 }
 
-static bool pix_quad_enabled() {
-  const char* e = getenv("ATOMAI_B200_PIX_QUAD");
-  return !(e && e[0] == '0');
-}
-
 int launch_conv_pix_quad(const ConvSimtParams& p, cudaStream_t stream) {
   const int64_t npix = (int64_t)p.N * p.H * p.W;
   int64_t blocks = (npix * 4 + 256 * 8 - 1) / (256 * 8);
@@ -956,8 +951,6 @@ int launch_wgrad_c1_tile(const WgradSimtParams& p, cudaStream_t stream) {
 
 // the tile kernels want dilation 1 and rows that fill most of the 64-pixel tile width
 static bool c1_tile_ok(int dil, int W) {
-  if (const char* e = getenv("ATOMAI_B200_C1_TILE"))
-    if (e[0] == '0') return false;
   const int tiles_w = (W + C1T_W - 1) / C1T_W;
   return dil == 1 && tiles_w * C1T_W - W <= W / 4;
 }
@@ -1197,7 +1190,7 @@ int ab_conv_simt_fwd(const ab_conv_t* d, const float* w, const float* bias, floa
       if (taps * Cin <= 64) {
         if (d->Cout == 8) return launch_conv_pix<8>(p, stream);
         if (d->Cout == 16 && taps == 1 && Cin <= 8 && p.S.nsrc == 1 && !p.S.s[0].pool && !d->out_nchw &&
-            ld_y % 4 == 0 && ((uintptr_t)y & 15) == 0 && pix_quad_enabled())
+            ld_y % 4 == 0 && ((uintptr_t)y & 15) == 0)
           return launch_conv_pix_quad(p, stream);
         if (d->Cout == 16) return launch_conv_pix<16>(p, stream);
         if (d->Cout % 32 == 0 && d->Cout <= 256 && !d->out_nchw) {
@@ -1247,8 +1240,7 @@ int ab_conv_simt_wgrad(const ab_conv_t* d, const float* dy, int ld_dy, float* dw
   if (p.S.Ctot <= 2 && d->ks_w == 1 && d->ks_h == 1) return launch_wgrad_small<16, 2, 1, 1>(p, stream);
   if (d->Cout <= 4 && d->ks_w == 1 && d->ks_h == 1 && p.S.Ctot == 16 && p.S.nsrc == 1 && !p.S.s[0].pool &&
       (p.S.s[0].ld & 3) == 0 && ((uintptr_t)p.S.s[0].ptr & 15) == 0 &&
-      (!p.S.s[0].scale || (((uintptr_t)p.S.s[0].scale | (uintptr_t)p.S.s[0].shift) & 15) == 0) &&
-      pix_quad_enabled())
+      (!p.S.s[0].scale || (((uintptr_t)p.S.s[0].scale | (uintptr_t)p.S.s[0].shift) & 15) == 0))
     return launch_wgrad_pix_quad(p, stream);
   if (d->Cout <= 4 && d->ks_w == 1 && d->ks_h == 1) return launch_wgrad_small<4, 16, 1, 1>(p, stream);
   if (d->Cout <= 4 && d->ks_w == 3 && d->ks_h == 3) return launch_wgrad_small<4, 4, 3, 3>(p, stream);

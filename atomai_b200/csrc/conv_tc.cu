@@ -844,9 +844,71 @@ int ab_pack_weights_tc(const float* w, int Cout, int Cin, int th, int tw, int mo
   return 0;
 }
 
+// Environment overrides of the tile-plan search, read once per plan (the tests set them between
+// calls to force every plan variant; tools/plan_ab.py and tools/show_plans.py sweep them).
+struct PlanKnobs {
+  int budget = 224 * 1024;   // ATOMAI_B200_SMEM_KB (64..224): shared memory the plan may use
+  int na4 = 3;               // ATOMAI_B200_NA4: operand-ring preference bits (see conv_tc_plan)
+  int min_nr = 4;            // ATOMAI_B200_MIN_NR (>= 2): fewest raw stages of a TMA plan
+  int attempt = -1, kc = 0;  // ATOMAI_B200_PLAN="<attempt>,<KC>": pin the weight mode / k-chunk
+  bool tma = true;           // ATOMAI_B200_TMA=0: register-staged loaders only
+  int res_na4 = -1;          // ATOMAI_B200_RES_NA4=0/1: resident n_a = 4 rule for no / every layer
+  int tma_min_kc = 16;       // ATOMAI_B200_TMA_KC8 (set): TMA plans may use 32-byte box rows
+  bool log = false;          // ATOMAI_B200_PLAN_LOG (set): print every plan to stderr
+};
+
+static PlanKnobs plan_knobs() {
+  PlanKnobs k;
+  if (const char* e = getenv("ATOMAI_B200_SMEM_KB")) {
+    const int kb = atoi(e);
+    if (kb >= 64 && kb <= 224) k.budget = kb * 1024;
+  }
+  if (const char* e = getenv("ATOMAI_B200_NA4")) k.na4 = atoi(e);
+  if (const char* e = getenv("ATOMAI_B200_MIN_NR")) k.min_nr = atoi(e) < 2 ? 2 : atoi(e);
+  if (const char* e = getenv("ATOMAI_B200_PLAN")) sscanf(e, "%d,%d", &k.attempt, &k.kc);
+  if (const char* e = getenv("ATOMAI_B200_TMA")) k.tma = e[0] != '0';
+  if (const char* e = getenv("ATOMAI_B200_RES_NA4")) k.res_na4 = e[0] == '1' ? 1 : 0;
+  if (getenv("ATOMAI_B200_TMA_KC8")) k.tma_min_kc = 8;
+  k.log = getenv("ATOMAI_B200_PLAN_LOG") != nullptr;
+  return k;
+}
+
+// Operand and weight stages of a k-chunk of KC channels: P = KC/4 planes of HP pixels x 16 B, the
+// plane stride padded so that the P planes start 128/P bytes apart mod 128 (spread over the
+// banks); x3 doubles both for the bf16 correction planes.  false: more 16-byte elements than the
+// register-staged loaders hold.
+struct Chunk { int KC, plane, a_stage, b_stage; };
+
+static bool chunk_stages(int HP, int KC, int Cout, int x3, Chunk* c) {
+  const int P = KC / 4;
+  if (HP * P > kMaxU * kGroupThreads) return false;
+  int plane = HP * 16;
+  const int want = (128 / P) % 128;
+  plane += ((want - plane % 128) + 128) % 128;
+  *c = {KC, plane, P * plane * (x3 ? 2 : 1), KC * Cout * 4 * (x3 ? 2 : 1)};
+  return true;
+}
+
+static void set_chunk(ConvTcParams* p, const Chunk& c) {
+  p->KC = c.KC; p->plane_bytes = c.plane; p->a_stage_bytes = c.a_stage; p->b_stage_bytes = c.b_stage;
+  p->corr_off = c.KC / 4 * c.plane;
+}
+
+// Shared memory of everything but the stages: the statistics / control block and, for resident
+// weights, the whole packed weight blob
+static int fixed_smem(const ConvTcParams& p, int stats_bytes, int resident) {
+  return stats_bytes + (resident ? (p.w_bytes + 127) & ~127 : 0);
+}
+
+static int plan_smem(const ConvTcParams& p, int stats_bytes) {
+  return fixed_smem(p, stats_bytes, p.w_resident) + p.n_a * p.a_stage_bytes + p.n_b * p.b_stage_bytes +
+         p.n_r * p.raw_bytes + (p.tma ? 128 : 0);
+}
+
 static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
   SrcSet S;
   if (ab_make_srcset(d, &S)) return 1;
+  const PlanKnobs k = plan_knobs();
   p->S = S;
   p->N = d->N; p->H = d->H; p->W = d->W; p->Cout = d->Cout;
   p->taps_h = d->ks_h; p->taps_w = d->ks_w; p->dil = d->dil;
@@ -857,48 +919,33 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
   p->x3 = d->math == AB_MATH_TF32X3 ? 1 : 0;
   p->w_bytes = taps * S.Ctot * d->Cout * 4 * (p->x3 ? 2 : 1);
   // 1 CTA / SM: 227 KB of dynamic shared memory are addressable (226 KB opted in below);
-  // ATOMAI_B200_SMEM_KB re-pins the plan budget (sweeps only)
-  int budget = 224 * 1024;
-  if (const char* e = getenv("ATOMAI_B200_SMEM_KB")) {
-    const int kb = atoi(e);
-    if (kb >= 64 && kb <= 224) budget = kb * 1024;
-  }
+  // the plan uses k.budget of them
   // Operand-ring preference.  Every pipeline owns n_a/2 operand stages; with n_a = 2 the loader
   // group and the consumer strictly alternate on a pipeline (stage -> MMA -> stage ...) and only
   // the *other* pipeline hides the hand-over.  Buying the deeper ring with 8-channel k-chunks does
   // not pay when the loaders are the heavy side (pooled sources, register-staged resident
   // layers), so pass 0 of the search only drops to KC = 8 for streamed-weight layers with plain
   // sources.
-  // bit 0: resident-weight plans prefer n_a = 4 over more raw TMA stages;
+  // k.na4 bit 0: resident-weight plans prefer n_a = 4 over more raw TMA stages;
   // bit 1: streamed-weight plans prefer n_a = 4 over a larger k-chunk / more weight stages.
-  int na4 = 3;
-  if (const char* e = getenv("ATOMAI_B200_NA4")) na4 = atoi(e);
-  // TMA mode needs at least this many raw stages (two rings of min_nr/2), else the plan stays
+  // TMA mode needs at least k.min_nr raw stages (two rings of min_nr/2), else the plan stays
   // register-staged: with one raw stage per pipeline every k-chunk pays the full HBM latency
-  int min_nr = 4;
-  if (const char* e = getenv("ATOMAI_B200_MIN_NR")) min_nr = atoi(e) < 2 ? 2 : atoi(e);
   bool any_pool = false;
   for (int i = 0; i < S.nsrc; ++i) any_pool = any_pool || S.s[i].pool != 0;
   const int stats_bytes = (((kNumEpiWarps * 2 + 1) * d->Cout * 4 + 127) & ~127) + kCtlBytes + 128;
   // Try, in order of preference: (resident weights, 1 sub-tile), (streamed weights, 2 sub-tiles
   // so that every weight stage feeds M = 256), (streamed, 1 sub-tile).
-  // tuning hooks (bring-up only): ATOMAI_B200_PLAN="<attempt>,<KC>" pins the plan search
-  int force_attempt = -1, force_kc = 0;
-  if (const char* e = getenv("ATOMAI_B200_PLAN")) sscanf(e, "%d,%d", &force_attempt, &force_kc);
-  const char* e_tma = getenv("ATOMAI_B200_TMA");      // "0" pins the register-staged loaders
-  const bool use_tma = !(e_tma && e_tma[0] == '0');
   bool ok = false;
   // Resident weights that leave only n_a = 2 vs streamed weights with n_a = 4: streaming wins only
   // where the weight ring gets deep enough to cover the L2 latency, i.e. for the two-source
   // decoder convolution onto <= 32 channels.  So: for that layer class a resident plan must reach
   // n_a = 4, else a streamed plan with >= 12 weight stages is preferred; the resident n_a = 2 plan
   // stays the fallback.  ATOMAI_B200_RES_NA4 = 0 disables, = 1 applies the rule to every layer.
-  const char* e_strict = getenv("ATOMAI_B200_RES_NA4");
   int strict0 = (p->x3 && S.nsrc == 2 && !any_pool && taps == 9 && d->Cout <= 32) ? 1 : 0;
-  if (e_strict) strict0 = e_strict[0] == '1' ? 1 : 0;
+  if (k.res_na4 >= 0) strict0 = k.res_na4;
   for (int strict = strict0; strict >= 0 && !ok; --strict)
   for (int attempt = 0; attempt < 3 && !ok; ++attempt) {
-    if (force_attempt >= 0 && attempt != force_attempt) continue;
+    if (k.attempt >= 0 && attempt != k.attempt) continue;
     const int resident = attempt == 0;
     const int sub = attempt == 1 ? 2 : 1;
     if (sub == 2 && (d->Cout > kMaxN / 2 || d->W <= kTileW)) continue;   // SUB * N accumulators
@@ -907,72 +954,54 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
     p->THp = kTileH + d->dil * (d->ks_h - 1);
     p->TWp = kTileW * sub + d->dil * (d->ks_w - 1);
     p->HP = p->THp * p->TWp;
-    // pass 0 (only when this weight mode prefers deep operand rings) accepts a k-chunk only if
-    // it leaves room for n_a = 4; pass 1 is the plain "largest k-chunk with n_a >= 2" search
-    const bool want4 = (na4 & (resident ? 1 : 2)) != 0;
-    for (int pass = want4 ? 0 : 1; pass < 2 && !ok; ++pass)
+    const int avail = k.budget - fixed_smem(*p, stats_bytes, resident);
+    // pass 0 (only when this weight mode prefers deep operand rings, or for a strict resident
+    // plan) accepts a k-chunk only if it leaves room for n_a = 4; pass 1 is the plain "largest
+    // k-chunk with n_a >= 2" search
+    for (int pass = (k.na4 & (resident ? 1 : 2)) ? 0 : 1; pass < 2 && !ok; ++pass)
     for (int KC = pick_kc(S.Ctot); KC >= 8 && !ok; KC >>= 1) {
-      if (S.Ctot % KC != 0) continue;
-      if (force_kc > 0 && KC != force_kc) continue;
-      const int P = KC / 4;
-      if (p->HP * P > kMaxU * kGroupThreads) continue;
-      int plane = p->HP * 16;
-      const int want = (128 / P) % 128;  // plane stride mod 128 spreading the P planes over banks
-      plane += ((want - plane % 128) + 128) % 128;
-      const int a_stage = P * plane * (p->x3 ? 2 : 1);    // x3: + the bf16 correction planes
-      const int need_a = pass == 0 ? 4 : 2;
-      if (pass == 0 && KC < 16 && (resident || any_pool)) continue;
-      int avail = budget - stats_bytes;
-      int n_b = 0, b_stage = KC * d->Cout * 4 * (p->x3 ? 2 : 1);
-      if (resident) {
-        avail -= (p->w_bytes + 127) & ~127;
-      } else {
+      const int need_a = pass == 0 || (strict && resident) ? 4 : 2;
+      Chunk c;
+      if (S.Ctot % KC != 0 || (k.kc > 0 && KC != k.kc) || !chunk_stages(p->HP, KC, d->Cout, p->x3, &c))
+        continue;
+      if (need_a == 4 && KC < 16 && (resident || any_pool)) continue;
+      int n_b = 0;
+      if (!resident) {
         // weight stages: cover the L2 latency, leave room for the activation stages
-        n_b = ((avail - need_a * a_stage) / b_stage) & ~1;      // two rings of n_b/2 stages
+        n_b = ((avail - need_a * c.a_stage) / c.b_stage) & ~1;      // two rings of n_b/2 stages
         if (n_b > kMaxBStages) n_b = kMaxBStages;
         if (n_b < (strict ? 12 : 4)) continue;
-        avail -= n_b * b_stage;
       }
-      int na = avail / a_stage;
+      const int na = (avail - n_b * c.b_stage) / c.a_stage;
       if (na < need_a) continue;
-      if (strict && resident && (na < 4 || KC < 16)) continue;
-      p->KC = KC; p->plane_bytes = plane; p->a_stage_bytes = a_stage; p->b_stage_bytes = b_stage;
-      p->corr_off = P * plane;
-      p->n_a = na > kMaxAStages ? kMaxAStages : na;
-      p->n_a &= ~1;   // two rings of n_a/2 stages
+      set_chunk(p, c);
+      p->n_a = (na > kMaxAStages ? kMaxAStages : na) & ~1;   // two rings of n_a/2 stages
       p->n_b = n_b; p->sub = sub; p->w_resident = resident;
       p->tma = 0; p->n_r = 0; p->raw_bytes = 0;
       ok = true;
     }
     // TMA mode (resident weights, un-pooled sources, sources split on a chunk boundary): choose
     // the (KC, operand stages, raw stages) with the most raw bytes in flight
-    if (ok && resident && use_tma && !S.s[0].pool && !(S.nsrc > 1 && S.s[1].pool)) {
+    if (ok && resident && k.tma && !S.s[0].pool && !(S.nsrc > 1 && S.s[1].pool)) {
       int best_bytes = 0;
-      const int tma_min_kc = getenv("ATOMAI_B200_TMA_KC8") ? 8 : 16;   // sweep hook: 32-byte box rows
-      for (int KC = pick_kc(S.Ctot); KC >= tma_min_kc; KC >>= 1) {
-        if (S.Ctot % KC != 0 || (S.nsrc > 1 && S.s[0].C % KC != 0)) continue;
-        if (force_kc > 0 && KC != force_kc) continue;
-        const int P = KC / 4;
-        if (p->HP * P > kMaxU * kGroupThreads) continue;
-        int plane = p->HP * 16;
-        const int want = (128 / P) % 128;
-        plane += ((want - plane % 128) + 128) % 128;
-        const int a_stage = P * plane * (p->x3 ? 2 : 1);
+      for (int KC = pick_kc(S.Ctot); KC >= k.tma_min_kc; KC >>= 1) {
+        Chunk c;
+        if (S.Ctot % KC != 0 || (S.nsrc > 1 && S.s[0].C % KC != 0) || (k.kc > 0 && KC != k.kc) ||
+            !chunk_stages(p->HP, KC, d->Cout, p->x3, &c))
+          continue;
         const int raw = p->HP * KC * 4;
         if (raw % 128 != 0) continue;
-        const int avail = budget - stats_bytes - ((p->w_bytes + 127) & ~127);
-        for (int na = 4; na >= ((na4 & 1) ? 4 : 2); na -= 2) {
-          int nr = ((avail - na * a_stage) / raw) & ~1;
+        for (int na = 4; na >= ((k.na4 & 1) ? 4 : 2); na -= 2) {
+          int nr = ((avail - na * c.a_stage) / raw) & ~1;
           if (nr > kMaxRStages) nr = kMaxRStages;
-          if (nr < min_nr) continue;
+          if (nr < k.min_nr) continue;
           // raw bytes in flight decide; with the n_a = 4 preference a double-buffered operand
           // ring outranks any number of raw stages
-          const int score = nr * raw + (na == 4 ? ((na4 & 1) ? (1 << 24) : 1) : 0);
+          const int score = nr * raw + (na == 4 ? ((k.na4 & 1) ? (1 << 24) : 1) : 0);
           if (score > best_bytes) {
             best_bytes = score;
-            p->KC = KC; p->plane_bytes = plane; p->a_stage_bytes = a_stage;
-            p->b_stage_bytes = KC * d->Cout * 4 * (p->x3 ? 2 : 1);
-            p->corr_off = P * plane; p->n_a = na; p->n_r = nr; p->raw_bytes = raw; p->tma = 1;
+            set_chunk(p, c);
+            p->n_a = na; p->n_r = nr; p->raw_bytes = raw; p->tma = 1;
           }
         }
       }
@@ -982,10 +1011,8 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
   p->num_tiles = d->N * p->tiles_h * p->tiles_w;
   p->n_chunks = S.Ctot / p->KC;
   AB_CHECK(p->plane_bytes / 16 < (1 << 14) && p->TWp < (1 << 14), "conv_tc: descriptor overflow");
-  *smem_bytes = stats_bytes + p->n_a * p->a_stage_bytes +
-                (p->w_resident ? ((p->w_bytes + 127) & ~127) : p->n_b * p->b_stage_bytes) +
-                p->n_r * p->raw_bytes + (p->tma ? 128 : 0);
-  if (getenv("ATOMAI_B200_PLAN_LOG"))
+  *smem_bytes = plan_smem(*p, stats_bytes);
+  if (k.log)
     fprintf(stderr,
             "conv_tc plan: %dx%d Cin=%d Cout=%d taps=%d x3=%d | resident=%d sub=%d KC=%d n_a=%d "
             "n_b=%d tma=%d n_r=%d a_stage=%d smem=%d\n",

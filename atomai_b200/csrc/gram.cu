@@ -9,7 +9,6 @@
 // tile kernel below.
 // RBF / Matern-2.5 / outputscale follow gpytorch's public kernel definitions as configured at
 // atomai/nets/gp.py:41-46 and :100-111 (gpytorch itself is not vendored by the reference).
-#include <cstdlib>
 #include "common.cuh"
 
 
@@ -167,11 +166,8 @@ extern "C" int atomai_b200_gram(const float* x1, const float* x2, const float* i
     const int x3 = math == AB_MATH_TF32X3;
     // rows of K per launch: as wide as the consumer's accumulator registers allow — wide N amortises
     // the A-operand reads and the per-tile handshakes
-    int blk = kColBlock;
-    if (const char* e = getenv("ATOMAI_B200_GRAM_BLOCK")) blk = atoi(e);
-    if (blk < 16 || blk > kColBlock || blk % 16 != 0) blk = kColBlock;
-    for (int r0 = 0; r0 < n1m; r0 += blk) {
-      const int rb = (n1m - r0) < blk ? (n1m - r0) : blk;
+    for (int r0 = 0; r0 < n1m; r0 += kColBlock) {
+      const int rb = (n1m - r0) < kColBlock ? (n1m - r0) : kColBlock;
       cd.Cout = rb;
       if (ab_pack_weights_tc(a + (int64_t)r0 * Kp, rb, Kp, 1, 1, AB_WMODE_FWD, x3, blob, st)) return 1;
       if (ab_conv_tc_fwd(&cd, blob, nullptr, K + (int64_t)r0 * ldk, -(int)ldk, nullptr, st)) return 1;

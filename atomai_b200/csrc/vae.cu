@@ -4,7 +4,6 @@
 //   * coord_latent fused with transform_coordinates (rVAE spatial decoder, first layer).
 // Reference call sites: atomai/nets/ed.py:64,273-274,503-505 (Linear), :672-687 (coord_latent),
 // atomai/utils/coords.py:47-83, atomai/models/dgm/rvae.py:118-145, atomai/nets/gp.py:14-26.
-#include <cstdlib>
 #include "common.cuh"
 
 namespace {
@@ -381,7 +380,7 @@ int atomai_b200_gemm(const float* A, int64_t a_sm, int64_t a_sk, const float* B,
 // y[B][O] = x[B][K] W[O][K]^T + b   — nn.Linear forward
 int atomai_b200_linear_fwd(const float* x, const float* w, const float* b, float* y, int B, int K,
                            int O, void* stream) {
-  if (skinny_ok(x, w, nullptr, B, K, O) && !getenv("ATOMAI_B200_NO_SKINNY")) {
+  if (skinny_ok(x, w, nullptr, B, K, O)) {
     // y = bias, then every k-slice CTA adds its partial sums
     bias_fill_kernel<<<(B * O + 255) / 256, 256, 0, (cudaStream_t)stream>>>(y, O, B, O, b);
     AB_LAUNCH_CHECK();
@@ -406,7 +405,7 @@ int atomai_b200_linear_fwd(const float* x, const float* w, const float* b, float
 int atomai_b200_linear_bwd(const float* x, const float* w, const float* dy, float* dx, float* dw,
                            float* db, int B, int K, int O, void* stream) {
   if (skinny_ok(x, w, dx, B, K, O) && ((uintptr_t)dw & 15) == 0 && (size_t)B * O * 4 <= 48 * 1024 &&
-      (dx || dw) && !getenv("ATOMAI_B200_NO_SKINNY")) {
+      (dx || dw)) {
     const int slices = (K + SK_KSB - 1) / SK_KSB;
     if (O <= 8)
       skinny_bwd_kernel<8><<<slices, SK_TB, (size_t)B * O * 4, (cudaStream_t)stream>>>(x, w, dy, dx, dw,

@@ -11,7 +11,6 @@ normalisation) and a *pending* 2x2 max-pool.  Consumers apply both while loading
 BatchNorm outputs, pooled tensors and torch.cat results are never written to HBM
 (atomai/nets/fcnn.py:117-142 materialises all of them).
 """
-import os
 from typing import List, Optional, Sequence, Union
 
 import torch
@@ -25,11 +24,6 @@ _MATH = {"mode": MATH_TF32X3, "wgrad_tc": True,   # default: the mode that meets
 
 
 _MODES = {"fp32": MATH_FP32, "tf32": MATH_TF32, "tf32x3": MATH_TF32X3}
-if os.environ.get("ATOMAI_B200_FUSE_UP", "0") == "1":     # A/B switch for benchmarking
-    _MATH["fuse_up"] = True
-
-
-_NO_POOLSTATS = os.environ.get("ATOMAI_B200_NO_POOLSTATS", "0") == "1"    # A/B switch (bring-up)
 
 
 def set_fusion(upsample: Optional[bool] = None) -> None:
@@ -369,7 +363,7 @@ class Tape:
         # forward, so last in backward): let the scatter kernel also produce the BatchNorm-backward
         # sums of the finished gradient; _acc_grad drops them again if something else follows.
         sums = None
-        if tgt.prod is not None and ops.pool_bwd_stats_ok(tgt.C) and not _NO_POOLSTATS:
+        if tgt.prod is not None and ops.pool_bwd_stats_ok(tgt.C):
             mean, invstd = tgt.prod
             sums = torch.zeros(2 * tgt.C, device=gp.device, dtype=torch.float64)
             ops.pool_bwd(gp, tgt.t, tgt.scale, tgt.shift, tgt.grad, acc, mean, invstd, sums)

@@ -638,46 +638,45 @@ def test_wgrad_exact(cuda, tag, layer, math):
 
 # ----------------------------------------------------------------------------- exact-fp32 kernels
 SIMT_FWD = [
-    ("c1_tile", L([1], 32, 40, 64), {}),
-    ("c1_16_dil2", L([1], 16, 24, 30, dil=2), {}),
-    ("c1_16_forced", L([1], 32, 40, 64), {"ATOMAI_B200_C1_TILE": "0"}),
-    ("pix4", L([16], 3, 20, 24, ks=1), {}),
-    ("pix4_3x3", L([S(8, aff=True)], 4, 13, 17), {}),
-    ("pix8", L([4], 8, 20, 24), {}),
-    ("pix_quad", L([8], 16, 20, 24, ks=1), {}),
-    ("pix16_no_quad", L([8], 16, 20, 24, ks=1), {"ATOMAI_B200_PIX_QUAD": "0"}),
-    ("pix16", L([4], 16, 13, 17), {}),
-    ("pix32", L([4], 64, 13, 17), {}),
-    ("generic", L([12], 24, 13, 21), {}),
-    ("generic_cat_pool", L([S(8, ops.SRC_POOL, aff=True), S(4)], 20, 10, 12), {}),
+    ("c1_tile", L([1], 32, 40, 64)),
+    ("c1_16_dil2", L([1], 16, 24, 30, dil=2)),
+    # 70 columns: the last 64-wide tile of conv_c1_tile would be mostly empty, so conv_c1<16> runs
+    ("c1_16_forced", L([1], 32, 40, 70)),
+    ("pix4", L([16], 3, 20, 24, ks=1)),
+    ("pix4_3x3", L([S(8, aff=True)], 4, 13, 17)),
+    ("pix8", L([4], 8, 20, 24)),
+    ("pix_quad", L([8], 16, 20, 24, ks=1)),
+    # pooled source: not a quad-lane shape, so conv_pix<16> runs
+    ("pix16_no_quad", L([S(8, ops.SRC_POOL)], 16, 20, 24, ks=1)),
+    ("pix16", L([4], 16, 13, 17)),
+    ("pix32", L([4], 64, 13, 17)),
+    ("generic", L([12], 24, 13, 21)),
+    ("generic_cat_pool", L([S(8, ops.SRC_POOL, aff=True), S(4)], 20, 10, 12)),
 ]
 SIMT_WGRAD = [
-    ("c1_tile", L([1], 16, 40, 64), {}),
-    ("c1_16", L([1], 16, 24, 30, dil=2), {}),
-    ("small_8_1_3x3", L([2], 8, 20, 24), {}),
-    ("small_16_1_1x3", L([2], 16, 1, 50, ks=(1, 3)), {}),
-    ("small_16_2_1x1", L([2], 16, 20, 24, ks=1), {}),
-    ("pix_quad", L([16], 4, 20, 24, ks=1), {}),
-    ("small_4_16_1x1", L([16], 3, 20, 24, ks=1), {"ATOMAI_B200_PIX_QUAD": "0"}),
-    ("small_4_4_3x3", L([8], 3, 20, 24), {}),
-    ("small_4_4_1x3", L([8], 3, 1, 50, ks=(1, 3)), {}),
-    ("generic", L([12], 24, 13, 21), {}),
+    ("c1_tile", L([1], 16, 40, 64)),
+    ("c1_16", L([1], 16, 24, 30, dil=2)),
+    ("small_8_1_3x3", L([2], 8, 20, 24)),
+    ("small_16_1_1x3", L([2], 16, 1, 50, ks=(1, 3))),
+    ("small_16_2_1x1", L([2], 16, 20, 24, ks=1)),
+    ("pix_quad", L([16], 4, 20, 24, ks=1)),
+    # pixel stride 17: not a quad-lane shape, so wgrad_small<4, 16, 1, 1> runs
+    ("small_4_16_1x1", L([S(16, pad=1)], 3, 20, 24, ks=1)),
+    ("small_4_4_3x3", L([8], 3, 20, 24)),
+    ("small_4_4_1x3", L([8], 3, 1, 50, ks=(1, 3))),
+    ("generic", L([12], 24, 13, 21)),
 ]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("tag,layer,env", SIMT_FWD, ids=[c[0] for c in SIMT_FWD])
-def test_simt_forward_exact(cuda, monkeypatch, tag, layer, env):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+@pytest.mark.parametrize("tag,layer", SIMT_FWD, ids=[c[0] for c in SIMT_FWD])
+def test_simt_forward_exact(cuda, tag, layer):
     run_fwd(layer, FP32, cuda, tag=tag, stats=True)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("tag,layer,env", SIMT_WGRAD, ids=[c[0] for c in SIMT_WGRAD])
-def test_simt_wgrad_exact(cuda, monkeypatch, tag, layer, env):
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+@pytest.mark.parametrize("tag,layer", SIMT_WGRAD, ids=[c[0] for c in SIMT_WGRAD])
+def test_simt_wgrad_exact(cuda, tag, layer):
     run_wgrad(layer, FP32, cuda, tag=tag)
 
 
@@ -688,12 +687,10 @@ def _twice(fn):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("tag,layer,env", SIMT_FWD, ids=[c[0] for c in SIMT_FWD])
-def test_simt_forward_reproducible(cuda, monkeypatch, tag, layer, env):
+@pytest.mark.parametrize("tag,layer", SIMT_FWD, ids=[c[0] for c in SIMT_FWD])
+def test_simt_forward_reproducible(cuda, tag, layer):
     """Normal data: two launches of each exact-fp32 forward branch give identical outputs and BN
     statistics (the statistics are ordered cross-CTA sums, not float atomics)."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
     g = _gen("simt_rep", tag)
     inp = _normal_inputs(layer, g, cuda)
     w = torch.randn((layer.cout, layer.ctot) + layer.ks, generator=g).to(cuda)
@@ -713,11 +710,9 @@ def test_simt_forward_reproducible(cuda, monkeypatch, tag, layer, env):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("tag,layer,env", SIMT_WGRAD, ids=[c[0] for c in SIMT_WGRAD])
-def test_simt_wgrad_reproducible(cuda, monkeypatch, tag, layer, env):
+@pytest.mark.parametrize("tag,layer", SIMT_WGRAD, ids=[c[0] for c in SIMT_WGRAD])
+def test_simt_wgrad_reproducible(cuda, tag, layer):
     """Normal data: two launches of each exact-fp32 weight-gradient branch give identical dW."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
     g = _gen("simt_rep_w", tag)
     inp = _normal_inputs(layer, g, cuda)
     _, dyv = nhwc_buf(torch.randn((layer.N, layer.cout, layer.H, layer.W), generator=g).double(), cuda)
@@ -868,7 +863,7 @@ def _normal_inputs(layer, g, dev):
     for s in layer.srcs:
         h, w = (2 * H, 2 * W) if s.tr == ops.SRC_POOL else (H, W)
         x = torch.randn((N, s.C, h, w), generator=g).double()
-        buf, view = nhwc_buf(x, dev)
+        buf, view = nhwc_buf(x, dev, s.pad)
         xr = x.to(dev)
         sc = sh = None
         if s.aff:

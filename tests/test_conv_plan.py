@@ -53,16 +53,20 @@ def test_every_shape_gets_a_plan(math):
     assert n >= 900
 
 
-@pytest.mark.parametrize("env", [{"ATOMAI_B200_NA4": "0", "ATOMAI_B200_SMEM_KB": "212", "ATOMAI_B200_MIN_NR": "2"},
-                                 {"ATOMAI_B200_RES_NA4": "1"}, {"ATOMAI_B200_RES_NA4": "0"},
-                                 {"ATOMAI_B200_TMA": "0"}, {"ATOMAI_B200_TMA_KC8": "1"}])
+KNOB_ENVS = [{"ATOMAI_B200_NA4": "0", "ATOMAI_B200_SMEM_KB": "212", "ATOMAI_B200_MIN_NR": "2"},
+             {"ATOMAI_B200_RES_NA4": "1"}, {"ATOMAI_B200_RES_NA4": "0"},
+             {"ATOMAI_B200_TMA": "0"}, {"ATOMAI_B200_TMA_KC8": "1"}]
+# (source channels, Cout, kernel size, pooled source) of the default Unet's tensor-core layers
+UNET = [([16], 32, 3, True), ([32], 32, 3, False), ([32], 64, 3, True), ([64], 64, 3, False),
+        ([64], 128, 3, True), ([128], 128, 3, False), ([128], 64, 1, False), ([64, 64], 64, 3, False),
+        ([64], 32, 1, False), ([32, 32], 32, 3, False), ([32], 16, 1, False), ([16, 16], 16, 3, False)]
+
+
+@pytest.mark.parametrize("env", KNOB_ENVS)
 def test_plan_knobs_keep_every_unet_layer_plannable(env, monkeypatch):
     for k, v in env.items():
         monkeypatch.setenv(k, v)
-    unet = [([16], 32, 3, True), ([32], 32, 3, False), ([32], 64, 3, True), ([64], 64, 3, False),
-            ([64], 128, 3, True), ([128], 128, 3, False), ([128], 64, 1, False), ([64, 64], 64, 3, False),
-            ([64], 32, 1, False), ([32, 32], 32, 3, False), ([32], 16, 1, False), ([16, 16], 16, 3, False)]
-    for cins, cout, ks, pool in unet:
+    for cins, cout, ks, pool in UNET:
         for hw in (32, 512):
             rc, _, _, smem = info(make_desc(cins, hw, cout, ks, 1, pool, ops.MATH_TF32X3))
             assert rc == 0 and smem <= OPT_IN, (env, cins, cout, smem)

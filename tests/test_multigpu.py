@@ -25,7 +25,7 @@ def test_two_rank_syncbn_equals_single_rank(cuda):
     # Forward quantities and the gradients of the last blocks agree to fp32 rounding.  The
     # gradients of the layers further upstream are an ill-conditioned function of the forward
     # (BatchNorm backward over few samples: ANY 1e-7 perturbation — another summation order, the
-    # tf32x3 mode, a second rank — moves them by several 1e-3, see tools/debug_x3_net.py), so the
+    # tf32x3 mode, a second rank — moves them by several 1e-3), so the
     # whole-model bound is 1e-2.
     assert out["loss_rel"] <= 1e-6, out
     assert out["running_mean_maxdiff"] <= 1e-6, out
