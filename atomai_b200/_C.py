@@ -17,7 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
            "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu",
-           "decomp.cu", "ed_ops.cu", "graph.cu"]
+           "decomp.cu", "ed_ops.cu", "graph.cu", "coords.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -34,12 +34,14 @@ JLAT_MAX_DISC = 64       # AB_JLAT_MAX_DISC
 JLAT_ALPHAS = 0
 JLAT_SAMPLE = 1
 GRAPH_MAX_RING = 32     # AB_GRAPH_MAX_RING
+COORDS_MAX_K = 32       # AB_COORDS_MAX_K
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile every CUDA source for sm_90a into libatomai_b200.so (in-tree)."""
     srcs = [os.path.join(CSRC, s) for s in SOURCES]
     deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "wgmma.cuh"),
+                   os.path.join(CSRC, "cellgrid.cuh"),
                    os.path.join(_HERE, "..", "include", "atomai_b200.h")]
     if not force and os.path.exists(LIB_PATH):
         t = os.path.getmtime(LIB_PATH)
@@ -177,6 +179,15 @@ SIGNATURES = {
     "atomai_b200_graph_hops": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "atomai_b200_graph_rings": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "atomai_b200_graph_ring_filter": (_i, [_vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "atomai_b200_coords_cells": (_i, [_vp, _i, C.POINTER(_d), _d, C.POINTER(_i64), _vp, _vp]),
+    "atomai_b200_coords_knn": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, C.POINTER(_d), _d,
+                                    C.POINTER(_i64), _i, _d, _vp, _vp, _vp]),
+    "atomai_b200_coords_ball": (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, C.POINTER(_d), _d,
+                                     C.POINTER(_i64), _d, _vp, _vp, _vp, _vp, _vp]),
+    "atomai_b200_coords_walk": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, C.POINTER(_d), _d,
+                                     C.POINTER(_i64), _d, _i64, _i64, _i64, _i64, _vp, _vp]),
+    "atomai_b200_coords_dbscan_roots": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "atomai_b200_coords_dbscan_labels": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_prob_mask": (_i, [_vp, _i, _i64, _i, _i, _f, _vp, _i, _vp, _vp]),
     "atomai_b200_gather_windows": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
     "atomai_b200_peak_refine": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),

@@ -5,7 +5,7 @@
 //   bonds       count pass: degree of every atom; fill pass: its CSR row, sorted ascending.  Atoms
 //               i != j bond when |p_i - p_j| (float64, unfused) <= cut[c_i][c_j]; the candidates
 //               come from the 3 x 3 (x 3) cells around the atom, found by binary search in the
-//               sorted keys, so the grid is never materialised.
+//               sorted keys, so the grid is never materialised (cellgrid.cuh).
 //   hops        one level of the bounded hop table: ball_k(u) = ball_{k-1}(u) U ball_{k-1}(w) + 1
 //               over the bonded w, as sorted rows of packed (id << 5 | hops) words.  Count pass and
 //               fill pass, like bonds.
@@ -21,6 +21,7 @@
 // Determinism: every output position comes from a count pass and a prefix sum of the caller; no
 // atomics decide any order, and a repeated call gives identical results.
 #include <math.h>
+#include "cellgrid.cuh"
 #include "common.cuh"
 
 namespace {
@@ -28,17 +29,6 @@ namespace {
 constexpr int kThreads = 128;
 constexpr int kHopBits = 5;  // hops <= 16 in the low bits of a packed hop-table word
 constexpr uint32_t kHopMask = (1u << kHopBits) - 1;
-
-struct Grid {
-  double lo[3];
-  double side;
-  int64_t n[3];
-};
-
-__device__ __forceinline__ int64_t cell_of(double p, double lo, double side, int64_t n) {
-  int64_t c = (int64_t)floor((p - lo) / side);
-  return c < 0 ? 0 : (c >= n ? n - 1 : c);
-}
 
 __global__ void __launch_bounds__(kThreads)
     graph_cell_keys_kernel(const double* __restrict__ pos, const int* __restrict__ frame, int N,
@@ -50,22 +40,6 @@ __global__ void __launch_bounds__(kThreads)
   const int64_t cy = cell_of(pos[3 * i + 1], g.lo[1], g.side, g.n[1]);
   const int64_t cz = cell_of(pos[3 * i + 2], g.lo[2], g.side, g.n[2]);
   keys[i] = ((f * g.n[2] + cz) * g.n[1] + cy) * g.n[0] + cx;
-}
-
-// first index t of the sorted keys with keys[t] >= k
-__device__ __forceinline__ int lower_key(const int64_t* __restrict__ keys, int N, int64_t k) {
-  int a = 0, b = N;
-  while (a < b) {
-    const int m = (a + b) >> 1;
-    if (keys[m] < k) a = m + 1;
-    else b = m;
-  }
-  return a;
-}
-
-__device__ __forceinline__ double dist3(const double* a, const double* b) {
-  const double dx = __dsub_rn(a[0], b[0]), dy = __dsub_rn(a[1], b[1]), dz = __dsub_rn(a[2], b[2]);
-  return sqrt(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
 }
 
 // rowptr == nullptr: deg[i] = number of bonds of i; else cols[rowptr[i] ...] = the bonded atoms,

@@ -765,6 +765,98 @@ def graph_ring_filter(off, lens, atoms, bptr, ball, keep) -> None:
                                               ptr(ball), ptr(keep), stream_ptr()))
 
 
+def coords_cells(pos, lo, side: float, dims, cells) -> None:
+    """cells (N, 3) int64: the grid cell of every row of pos (N, 3) float64, as graph_cell_keys
+    bins it."""
+    N = pos.shape[0]
+    assert pos.dtype == torch.float64 and pos.shape == (N, 3) and pos.is_contiguous()
+    assert cells.dtype == torch.int64 and cells.shape == (N, 3) and cells.is_contiguous()
+    lo_, dims_ = _grid_args(lo, dims)
+    check(lib().atomai_b200_coords_cells(ptr(pos), N, lo_, float(side), dims_, ptr(cells),
+                                         stream_ptr()))
+
+
+def coords_knn(qpos, qcell, qframe, pos, keys, perm, foff, lo, side: float, dims, k: int,
+               ub: float, oidx, odist) -> None:
+    """The k nearest rows of pos (N, 3) float64 with distance < ub to every query (qpos (Q, 3),
+    in cells qcell (Q, 3) int64), within the query's frame qframe (Q,) int32 whose atoms are the
+    sorted keys foff[f]:foff[f + 1] (both None: one frame).  oidx (Q, k) int32 / odist (Q, k)
+    float64 ascending, -1 / inf where fewer are found; an equal distance goes to the lower index."""
+    Q, N = qpos.shape[0], pos.shape[0]
+    assert qpos.dtype == pos.dtype == odist.dtype == torch.float64
+    assert qpos.shape == (Q, 3) and pos.shape == (N, 3) and qpos.is_contiguous() and pos.is_contiguous()
+    assert qcell.dtype == torch.int64 and qcell.shape == (Q, 3) and qcell.is_contiguous()
+    assert keys.dtype == perm.dtype == torch.int64 and keys.shape == perm.shape == (N,)
+    assert (qframe is None) == (foff is None)
+    assert qframe is None or (qframe.dtype == torch.int32 and qframe.shape == (Q,)
+                              and foff.dtype == torch.int64)
+    assert oidx.dtype == torch.int32 and oidx.shape == odist.shape == (Q, k)
+    assert oidx.is_contiguous() and odist.is_contiguous()
+    lo_, dims_ = _grid_args(lo, dims)
+    check(lib().atomai_b200_coords_knn(ptr(qpos), ptr(qcell), ptr(qframe), Q, ptr(pos), N,
+                                       ptr(keys), ptr(perm), ptr(foff), lo_, float(side), dims_,
+                                       int(k), float(ub), ptr(oidx), ptr(odist), stream_ptr()))
+
+
+def coords_ball(qpos, qcell, pos, keys, perm, lo, side: float, dims, rmax: float, rowptr=None,
+                oidx=None, odist=None, cnt=None) -> None:
+    """Rows of pos with distance < rmax (<= side) of every query.  rowptr None: cnt (Q,) int64 =
+    their number; else oidx (int32) / odist (float64)[rowptr[i]:rowptr[i + 1]] = them, in scan
+    order."""
+    Q, N = qpos.shape[0], pos.shape[0]
+    assert qpos.dtype == pos.dtype == torch.float64 and qpos.shape == (Q, 3) and pos.shape == (N, 3)
+    assert qpos.is_contiguous() and pos.is_contiguous()
+    assert qcell.dtype == torch.int64 and qcell.shape == (Q, 3) and qcell.is_contiguous()
+    assert keys.dtype == perm.dtype == torch.int64 and keys.shape == perm.shape == (N,)
+    if rowptr is None:
+        assert cnt.dtype == torch.int64 and cnt.shape == (Q,)
+    else:
+        assert rowptr.dtype == torch.int64 and rowptr.shape == (Q + 1,)
+        assert oidx.dtype == torch.int32 and odist.dtype == torch.float64
+    lo_, dims_ = _grid_args(lo, dims)
+    check(lib().atomai_b200_coords_ball(ptr(qpos), ptr(qcell), Q, ptr(pos), N, ptr(keys), ptr(perm),
+                                        lo_, float(side), dims_, float(rmax), ptr(rowptr), ptr(oidx),
+                                        ptr(odist), ptr(cnt), stream_ptr()))
+
+
+def coords_walk(start, scell, pos, pcell, keys, perm, foff, lo, side: float, dims, rmax: float,
+                H: int, W: int, half: int, r: int, out) -> None:
+    """One walk per start (S, 3) through the frames of pos (atoms of frame f: sorted keys
+    foff[f]:foff[f + 1]): out (S, F, 4) int32 = (f, atom, row0, col0) of each step, or
+    (f, -1, -1, -1) where the frame is skipped (no atom with d < rmax, or numpy's slice
+    [cx - half : cx + half, cy - half : cy + half] of an H x W image is not r x r)."""
+    S, N, F = start.shape[0], pos.shape[0], foff.shape[0] - 1
+    assert start.dtype == pos.dtype == torch.float64 and start.shape == (S, 3) and pos.shape == (N, 3)
+    assert scell.dtype == pcell.dtype == torch.int64 and scell.shape == (S, 3) and pcell.shape == (N, 3)
+    assert keys.dtype == perm.dtype == foff.dtype == torch.int64 and keys.shape == perm.shape == (N,)
+    assert out.dtype == torch.int32 and out.shape == (S, F, 4) and out.is_contiguous()
+    lo_, dims_ = _grid_args(lo, dims)
+    check(lib().atomai_b200_coords_walk(ptr(start), ptr(scell), S, ptr(pos), ptr(pcell), ptr(keys),
+                                        ptr(perm), ptr(foff), F, lo_, float(side), dims_,
+                                        float(rmax), int(H), int(W), int(half), int(r), ptr(out),
+                                        stream_ptr()))
+
+
+def coords_dbscan_roots(rowptr, cols, min_samples: int, parent, flag) -> None:
+    """parent (N,) int32: the least core index of the component of every core point of the CSR
+    neighbourhoods (row length + 1 >= min_samples), -1 for the others.  flag: 1 int32 scratch."""
+    N = rowptr.shape[0] - 1
+    assert rowptr.dtype == torch.int64 and cols.dtype == torch.int32
+    assert parent.dtype == flag.dtype == torch.int32 and parent.shape == (N,)
+    check(lib().atomai_b200_coords_dbscan_roots(ptr(rowptr), ptr(cols), N, int(min_samples),
+                                                ptr(parent), ptr(flag), stream_ptr()))
+
+
+def coords_dbscan_labels(rowptr, cols, parent, rank, labels) -> None:
+    """labels (N,) int64 = rank[root] of every core point's root and of the least root among a
+    border point's core neighbours, -1 for noise."""
+    N = rowptr.shape[0] - 1
+    assert rowptr.dtype == rank.dtype == labels.dtype == torch.int64 and cols.dtype == torch.int32
+    assert parent.dtype == torch.int32 and parent.shape == rank.shape == labels.shape == (N,)
+    check(lib().atomai_b200_coords_dbscan_labels(ptr(rowptr), ptr(cols), N, ptr(parent), ptr(rank),
+                                                 ptr(labels), stream_ptr()))
+
+
 def peak_refine(stack, atoms, dmax: int, popt, info, nfev=None) -> None:
     """One lmdif fit of a rotated 2-D Gaussian per int32 row (frame, row0, col0, d) of `atoms` to
     the windows of the fp32 (n, H, W) `stack`: popt (K, 7) float64, info / nfev (K,) int32."""

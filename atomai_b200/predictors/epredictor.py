@@ -9,6 +9,7 @@ from typing import Dict, Tuple, Type, Union
 import numpy as np
 import torch
 
+from ..utils.coords import cluster_coord
 from ..utils.nn import get_downsample_factor
 from ..utils.preproc import torch_format_image, torch_format_spectra
 from .predictor import BasePredictor, Locator
@@ -152,28 +153,11 @@ class EnsemblePredictor(BasePredictor):
         return prediction_mean.transpose(c_tr), prediction_var.transpose(c_tr)
 
 
-def cluster_coord(coord_class_dict, eps: float, min_samples: int = 10):
-    """Collapses the coordinates of a stack onto the xy plane and clusters them with DBSCAN
-    (atomai/utils/coords.py:304-347): returns (points per cluster, cluster means, cluster
-    variances); like the reference, the first entry of np.unique(labels) is skipped."""
-    from sklearn import cluster
-    coordinates_all = np.empty((0, 3))
-    for k in range(len(coord_class_dict)):
-        coordinates_all = np.append(coordinates_all, coord_class_dict[k], axis=0)
-    labels = cluster.DBSCAN(eps=eps, min_samples=min_samples).fit(coordinates_all[:, :2]).labels_
-    clusters, clusters_var, clusters_mean = [], [], []
-    for lab in np.unique(labels)[1:]:
-        coord = coordinates_all[np.where(labels == lab)]
-        clusters.append(coord)
-        clusters_mean.append(np.mean(coord[:, :2], axis=0))
-        clusters_var.append(np.var(coord[:, :2], axis=0))
-    return clusters, np.array(clusters_mean), np.array(clusters_var)
-
-
 def ensemble_locate(nn_output_ensemble: np.ndarray, **kwargs: Dict) -> Tuple[np.ndarray]:
     """Coordinates for each ensemble member's prediction and their per-atom mean / variance
     (atomai/predictors/epredictor.py:238-267): nn_output_ensemble is (n_models, n_images, h, w,
-    c); kwargs eps (DBSCAN radius, default 0.5), threshold (Locator threshold, default 0.5)."""
+    c); kwargs eps (DBSCAN radius, default 0.5), threshold (Locator threshold, default 0.5).  The
+    members' coordinates are clustered by utils.coords.cluster_coord (DBSCAN on the GPU)."""
     eps = kwargs.get("eps", 0.5)
     thresh = kwargs.get("threshold", 0.5)
     coord_mean_all, coord_var_all = {}, {}

@@ -1,5 +1,7 @@
-from .coords import (find_com, get_intensities, get_lengthscale_constraints, get_nn_distances_, grid2xy,
-                     imcoordgrid, peak_refinement, remove_edge_coord, transform_coordinates)
+from .coords import (cluster_coord, compare_coordinates, find_com, find_coord_clusters,
+                     get_intensities, get_lengthscale_constraints, get_nn_distances,
+                     get_nn_distances_, grid2xy, imcoordgrid, map_bonds, peak_refinement,
+                     remove_edge_coord, subimg_trajectories, transform_coordinates)
 from .graphx import (Graph, Node, filter_subgraphs, filter_subgraphs_, find_cycle_clusters,
                      find_cycles, get_interatomic_r, plot_graph)
 from .img import (crop_borders, cv_thresh, extract_random_subimages, extract_subimages,

@@ -566,6 +566,51 @@ int atomai_b200_graph_ring_filter(const int64_t* off, const int* lens, const int
                                   int64_t R, const int64_t* bptr, const uint32_t* ball,
                                   unsigned char* keep, void* stream);
 
+/* ---- neighbour searches of atomic coordinates (csrc/coords.cu) ------------------------------
+ * pos: N x 3 float64, binned by graph_cell_keys into the grid (lo_host, side, dims_host; HOST
+ * arrays) with keys / perm the stably sorted keys and the atom of each.  foff (F + 1 int64) holds
+ * the first sorted key of every frame; the atoms of a batch are stored frame by frame.  Distances
+ * are float64, unfused; an equal distance goes to the lower index.  Every query comes with its
+ * cell (3 int64), which coords_cells writes for N points of the same grid.
+ * knn: the k nearest atoms with d < ub (ub = +inf: no bound) of query i (qpos Q x 3) in frame
+ *   qframe[i] (nullable with foff = NULL: one frame of N atoms): oidx / odist (Q x k) ascending,
+ *   -1 / +inf where fewer are found.  1 <= k <= AB_COORDS_MAX_K.
+ * ball: the atoms with d < rmax of every query (side >= rmax, one frame).  rowptr == NULL:
+ *   cnt[i] = their number; else oidx / odist[rowptr[i] ...] = them, in scan order.
+ * walk: for start s (start S x 3 with z = 0, cells scell) and frame f = 0 ... F-1 (atom cells
+ *   pcell): the nearest atom j of
+ *   frame f with d < rmax to the walk's position; out[(s F + f) 4 ...] = (f, j, row0, col0) when
+ *   numpy's slice [cx - half : cx + half, cy - half : cy + half] of an H x W image, cx, cy the
+ *   half-to-even rounded (x, y) of j, is r x r (the walk then moves to j), else (f, -1, -1, -1).
+ * dbscan_roots: parent[i] = the least core index of i's component for a core point of the CSR
+ *   (rowptr, cols) neighbourhoods (row length + 1 >= min_samples), -1 otherwise.  flag: 1 int of
+ *   device scratch.  Synchronises the stream once per round.
+ * dbscan_labels: labels[i] = rank[root] of i's root, or of the least root among a border point's
+ *   core neighbours, else -1. */
+#define AB_COORDS_MAX_K 32
+int atomai_b200_coords_cells(const double* pos, int N, const double* lo_host, double side,
+                             const int64_t* dims_host, int64_t* cells, void* stream);
+int atomai_b200_coords_knn(const double* qpos, const int64_t* qcell, const int* qframe, int Q,
+                           const double* pos, int N, const int64_t* keys, const int64_t* perm,
+                           const int64_t* foff, const double* lo_host, double side,
+                           const int64_t* dims_host, int k, double ub, int* oidx, double* odist,
+                           void* stream);
+int atomai_b200_coords_ball(const double* qpos, const int64_t* qcell, int Q, const double* pos,
+                            int N, const int64_t* keys, const int64_t* perm,
+                            const double* lo_host, double side, const int64_t* dims_host,
+                            double rmax, const int64_t* rowptr, int* oidx, double* odist,
+                            int64_t* cnt, void* stream);
+int atomai_b200_coords_walk(const double* start, const int64_t* scell, int S, const double* pos,
+                            const int64_t* pcell, const int64_t* keys, const int64_t* perm,
+                            const int64_t* foff, int F, const double* lo_host, double side,
+                            const int64_t* dims_host, double rmax, int64_t H, int64_t W,
+                            int64_t half, int64_t r, int* out, void* stream);
+int atomai_b200_coords_dbscan_roots(const int64_t* rowptr, const int* cols, int N,
+                                    int min_samples, int* parent, int* flag, void* stream);
+int atomai_b200_coords_dbscan_labels(const int64_t* rowptr, const int* cols, int N,
+                                     const int* parent, const int64_t* rank, int64_t* labels,
+                                     void* stream);
+
 /* ---- multi-GPU: small all-reduce over NVLink peer memory (csrc/p2p.cu) -----------------
  * Every rank exposes a zero-initialised mailbox (atomai_b200_p2p_data_bytes) and flag buffer
  * (atomai_b200_p2p_flag_bytes) to its peers (CUDA IPC: atomai_b200_ipc_export gives the 64-byte
