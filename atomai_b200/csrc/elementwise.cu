@@ -248,6 +248,16 @@ __device__ __forceinline__ void up_src(int o, int n, int& i0, int& i1, float& l1
   i1 = i0 + 1 < n ? i0 + 1 : n - 1;
 }
 
+// (1-lh)((1-lw)a + lw b) + lh((1-lw)c + lw d), with the FMAs spelled out: each sum is one FMA of
+// its first product onto the rounded second product.  Left to the compiler, the contraction
+// differed between the two kernels below (whether lh / lw are constants or not); this is the
+// form the 2x2-block kernel has always computed, and both kernels now give its bits.
+__device__ __forceinline__ float bil_mix(float a, float b, float c, float d, float lh, float lw) {
+  const float top = fmaf(1.f - lw, a, __fmul_rn(lw, b));
+  const float bot = fmaf(1.f - lw, c, __fmul_rn(lw, d));
+  return fmaf(1.f - lh, top, __fmul_rn(lh, bot));
+}
+
 __global__ void upsample_fwd_kernel(const float* __restrict__ x, int ld_x, float* __restrict__ y,
                                     int ld_y, int N, int h, int w, int C, int bilinear) {
   const int H = 2 * h, W = 2 * w;
@@ -268,7 +278,7 @@ __global__ void upsample_fwd_kernel(const float* __restrict__ x, int ld_x, float
       up_src(ow, w, w0, w1, lw);
       const float x00 = xb[((int64_t)h0 * w + w0) * ld_x], x01 = xb[((int64_t)h0 * w + w1) * ld_x];
       const float x10 = xb[((int64_t)h1 * w + w0) * ld_x], x11 = xb[((int64_t)h1 * w + w1) * ld_x];
-      v = (1.f - lh) * ((1.f - lw) * x00 + lw * x01) + lh * ((1.f - lw) * x10 + lw * x11);
+      v = bil_mix(x00, x01, x10, x11, lh, lw);
     } else {
       v = xb[((int64_t)(oh >> 1) * w + (ow >> 1)) * ld_x];
     }
@@ -310,7 +320,8 @@ __global__ void upsample_bwd_kernel(const float* __restrict__ dy, int ld_dy, flo
       }
     } else {
       const int64_t b0 = ((int64_t)(2 * ih) * W + 2 * iw) * ld_dy;
-      acc = db[b0] + db[b0 + ld_dy] + db[b0 + (int64_t)W * ld_dy] + db[b0 + (int64_t)W * ld_dy + ld_dy];
+      // (top pair) + (bottom pair), as the float4 kernel sums them
+      acc = (db[b0] + db[b0 + ld_dy]) + (db[b0 + (int64_t)W * ld_dy] + db[b0 + (int64_t)W * ld_dy + ld_dy]);
     }
     dx[(((int64_t)n * h + ih) * w + iw) * ld_dx + c] = acc;
   }
@@ -721,12 +732,9 @@ __global__ void __launch_bounds__(kT) upsample_fwd_blk_kernel(const float* __res
     const float4 pm = ld4(rp + (size_t)wm * ld_x), p0 = ld4(rp + (size_t)iw * ld_x), pp = ld4(rp + (size_t)wp * ld_x);
     // even output index 2i: (x[i-1], x[i], l = 0.75)  [i = 0: l = 0];  odd 2i+1: (x[i], x[i+1], l = 0.25)
     const float lhe = ih > 0 ? 0.75f : 0.f, lwe = iw > 0 ? 0.75f : 0.f;
-    auto mix = [](float a, float b, float c, float d, float lh, float lw) {
-      return (1.f - lh) * ((1.f - lw) * a + lw * b) + lh * ((1.f - lw) * c + lw * d);
-    };
     auto mix4 = [&](float4 a, float4 b, float4 c, float4 d, float lh, float lw) {
-      return make_float4(mix(a.x, b.x, c.x, d.x, lh, lw), mix(a.y, b.y, c.y, d.y, lh, lw),
-                         mix(a.z, b.z, c.z, d.z, lh, lw), mix(a.w, b.w, c.w, d.w, lh, lw));
+      return make_float4(bil_mix(a.x, b.x, c.x, d.x, lh, lw), bil_mix(a.y, b.y, c.y, d.y, lh, lw),
+                         bil_mix(a.z, b.z, c.z, d.z, lh, lw), bil_mix(a.w, b.w, c.w, d.w, lh, lw));
     };
     *reinterpret_cast<float4*>(yb) = mix4(mm, m0, zm, z0, lhe, lwe);
     *reinterpret_cast<float4*>(yb + ld_y) = mix4(m0, mp, z0, zp, lhe, 0.25f);

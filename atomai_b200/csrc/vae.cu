@@ -17,7 +17,7 @@ struct GemmParams {
   int M, N, K;
   const float* bias;
   int act; float slope;
-  int accumulate;  // C += result (plain add when split_k == 1, atomics otherwise)
+  int accumulate;  // C += act(A.B + bias) (plain add when split_k == 1, atomics otherwise)
   int split_k, k_per_split;
 };
 
@@ -79,7 +79,11 @@ __global__ void __launch_bounds__(GT) gemm_kernel(const GemmParams p) {
       if (n >= p.N) continue;
       float* c = p.C + (int64_t)m * p.c_sm + n;
       if (p.split_k > 1) {
-        atomicAdd(c, acc[i][j]);
+        // C already holds the bias (bias_fill_kernel) unless accumulating; then the first K
+        // slice adds it, so that C += A.B + bias on every path
+        float v = acc[i][j];
+        if (p.accumulate && p.bias && blockIdx.z == 0) v += __ldg(p.bias + n);
+        atomicAdd(c, v);
       } else {
         float v = acc[i][j] + (p.bias ? __ldg(p.bias + n) : 0.f);
         v = act_f(v, p.act, p.slope);
@@ -350,7 +354,7 @@ extern "C" {
 int atomai_b200_gemm(const float* A, int64_t a_sm, int64_t a_sk, const float* B, int64_t b_sk,
                      int64_t b_sn, float* C, int64_t c_sm, int M, int N, int K, const float* bias,
                      int act, float slope, int accumulate, int split_k, void* stream) {
-  AB_CHECK(A && B && C, "gemm: null pointer");
+  AB_CHECK(C && (K == 0 || (A && B)), "gemm: null pointer");   // K = 0: C (+)= act(bias)
   AB_CHECK(M >= 0 && N >= 0 && K >= 0, "gemm: negative dims");
   if (M == 0 || N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;

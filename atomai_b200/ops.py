@@ -341,6 +341,9 @@ def add_slice(src, dst, accumulate) -> None:
 
 
 def dilated_sum(a_list, scale_list, shift_list, slope, out) -> None:
+    # the kernel reads every layer and writes `out` as dense arrays of out.numel() elements
+    assert out.is_contiguous() and all(t.is_contiguous() and t.numel() == out.numel()
+                                       for t in a_list), "dilated_sum: dense tensors expected"
     n = len(a_list)
     arr = C.c_void_p * n
     a = arr(*[t.data_ptr() for t in a_list])

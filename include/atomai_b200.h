@@ -307,8 +307,11 @@ int atomai_b200_linear_bwd(const float* x, const float* w, const float* dy, floa
                            float* dw, float* db, int B, int K, int O, void* stream);
 /* General strided fp32 GEMM used by the skinny/odd-shaped Linear layers:
  *   C[m][n] (+)= act( sum_k A[m*a_sm + k*a_sk] * B[k*b_sk + n*b_sn] + bias[n] )
- * split_k > 1 distributes K over CTAs with atomic accumulation (then act must be
- * identity and C pre-initialised, e.g. with the bias). */
+ * accumulate = 1 adds to C (C += act(A.B + bias)), 0 overwrites it.  split_k > 1
+ * distributes K over CTAs with atomic accumulation (then act must be identity); the
+ * effective split also depends on K (K <= 16 always runs as one split), and both
+ * give the same result up to the order of the fp32 sums.  A and B may be NULL when
+ * K = 0 (C (+)= act(bias)). */
 int atomai_b200_gemm(const float* A, int64_t a_sm, int64_t a_sk, const float* B, int64_t b_sk,
                      int64_t b_sn, float* C, int64_t c_sm, int M, int N, int K, const float* bias,
                      int act, float slope, int accumulate, int split_k, void* stream);
