@@ -169,12 +169,6 @@ __global__ void __launch_bounds__(kT) aug_pass_c(float* __restrict__ y, int64_t 
     y[e] = (y[e] - lo) * inv;
 }
 
-int grid_for(int64_t n) {
-  int64_t g = (n + kT - 1) / kT;
-  const int64_t cap = (int64_t)ab_num_sms() * 16;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 }  // namespace
 
 extern "C" int atomai_b200_augment(const float* x, float* y, float* scratch, const int64_t* lab_in,
@@ -188,12 +182,12 @@ extern "C" int atomai_b200_augment(const float* x, float* y, float* scratch, con
   const int64_t total = (int64_t)n * h * w;
   const float init[2] = {3.4e38f, -3.4e38f};
   AB_CUDA(cudaMemcpyAsync(minmax, init, sizeof(init), cudaMemcpyHostToDevice, st));
-  aug_pass_a<<<grid_for(total), kT, 0, st>>>(x, scratch, lab_in, lab_out, params, row_shift, n, h, w,
+  aug_pass_a<<<ab_grid(total, kT, 16), kT, 0, st>>>(x, scratch, lab_in, lab_out, params, row_shift, n, h, w,
                                             in_min, 1.f / (in_max - in_min), seed);
   AB_LAUNCH_CHECK();
-  aug_pass_b<<<grid_for(total), kT, 0, st>>>(scratch, y, params, n, h, w, minmax);
+  aug_pass_b<<<ab_grid(total, kT, 16), kT, 0, st>>>(scratch, y, params, n, h, w, minmax);
   AB_LAUNCH_CHECK();
-  aug_pass_c<<<grid_for(total), kT, 0, st>>>(y, total, minmax);
+  aug_pass_c<<<ab_grid(total, kT, 16), kT, 0, st>>>(y, total, minmax);
   AB_LAUNCH_CHECK();
   return 0;
 }

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <initializer_list>
+#include <type_traits>
 #include "../../include/atomai_b200.h"
 
 // ---------------------------------------------------------------- host errors
@@ -28,6 +30,14 @@ void ab_set_error(const char* fmt, ...);
 #define AB_LAUNCH_CHECK() AB_CUDA(cudaGetLastError())
 
 int ab_num_sms();  // cached SM count of the current device
+// CTAs of a grid-stride launch over `items` at `per_cta` items per CTA, at most `ctas_per_sm` per
+// SM: a function of the shape and the SM count only, so ordered cross-CTA sums are reproducible
+inline int ab_grid(int64_t items, int64_t per_cta, int ctas_per_sm) {
+  int64_t b = (items + per_cta - 1) / per_cta;
+  const int64_t cap = (int64_t)ab_num_sms() * ctas_per_sm;
+  if (b > cap) b = cap;
+  return b < 1 ? 1 : (int)b;
+}
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per device: `done` is a per-kernel table
 // indexed by the current device (set once per device, benign if two threads race)
 int ab_optin_smem(const void* func, int bytes, unsigned char* done);
@@ -68,6 +78,85 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// ---------------------------------------------------------------- W channels per thread
+// The memory-bound NHWC kernels have one body for two widths: W = 4 consecutive channels per
+// thread (one 16-byte load or store) when vec_ok() holds, W = 1 for any other layout.  The
+// arithmetic is written per lane, so both widths compute the same expression per element.
+template <int W>
+struct alignas(4 * W) Lanes {
+  float v[W];
+  __device__ __forceinline__ float& operator[](int k) { return v[k]; }
+  __device__ __forceinline__ float operator[](int k) const { return v[k]; }
+};
+template <int W>
+__device__ __forceinline__ Lanes<W> lanes_fill(float x) {
+  Lanes<W> r;
+#pragma unroll
+  for (int k = 0; k < W; ++k) r[k] = x;
+  return r;
+}
+// read-only input.  W = 4 through __ldg (the non-coherent cache); W = 1 a plain load, which the
+// compiler sends the same way for const __restrict__ pointers.  An explicit __ldg there keeps it
+// from unrolling the scalar grid-stride loops, which made them up to 9% slower on an H100.
+template <int W>
+__device__ __forceinline__ Lanes<W> lanes_ld(const float* p) {
+  if constexpr (W == 4) {
+    const float4 t = __ldg(reinterpret_cast<const float4*>(p));
+    return {{t.x, t.y, t.z, t.w}};
+  } else {
+    return {{*p}};
+  }
+}
+// output (or an accumulated input): plain loads and stores
+template <int W>
+__device__ __forceinline__ Lanes<W>& lanes_at(float* p) {
+  return *reinterpret_cast<Lanes<W>*>(p);
+}
+// Flat index over (pixel, group of W channels) -> pixel and its first channel.  W = 4: 32-bit
+// (vec_ok bounds the item count), with shift / mask when C/4 is a power of two.  W = 1: 64-bit,
+// so the scalar path takes tensors of 2^31 elements and more.
+template <int W>
+struct ChanIdx;
+template <>
+struct ChanIdx<4> {
+  using I = uint32_t;
+  int C4;
+  int shift;  // log2(C4) or -1
+  explicit ChanIdx(int C) : C4(C / 4), shift(-1) {
+    for (int s = 0; s < 12; ++s) if ((1 << s) == C4) shift = s;
+  }
+  __device__ __forceinline__ void split(uint32_t i, uint32_t& pix, int& c) const {
+    int c4;
+    if (shift >= 0) { pix = i >> shift; c4 = (int)(i & (uint32_t)(C4 - 1)); }
+    else { pix = i / (uint32_t)C4; c4 = (int)(i - pix * (uint32_t)C4); }
+    c = c4 * 4;
+  }
+};
+template <>
+struct ChanIdx<1> {
+  using I = int64_t;
+  int C;
+  explicit ChanIdx(int C_) : C(C_) {}
+  __device__ __forceinline__ void split(int64_t i, int64_t& pix, int& c) const {
+    c = (int)(i % C);
+    pix = i / C;
+  }
+};
+// the float4 path: C % 4 == 0, fewer than 2^31 groups of 4, every non-null pointer 16-byte
+// aligned and every pixel stride a multiple of 4
+inline bool vec_ok(int C, std::initializer_list<const void*> ptrs, std::initializer_list<int> lds,
+                   int64_t total4) {
+  if (C % 4 != 0 || total4 >= (int64_t)1 << 31) return false;
+  for (auto p : ptrs) if (p && ((uintptr_t)p & 15)) return false;
+  for (auto l : lds) if (l % 4 != 0) return false;
+  return true;
+}
+// host: f(std::integral_constant<int, W>{}) with W = 4 when `vec`, else W = 1
+template <class F>
+inline int by_width(bool vec, F f) {
+  return vec ? f(std::integral_constant<int, 4>{}) : f(std::integral_constant<int, 1>{});
 }
 
 // Counter-based RNG shared by dropout and the Gumbel noise of the joint VAEs: a 64-bit mix of the

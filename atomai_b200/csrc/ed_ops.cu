@@ -14,13 +14,6 @@ namespace {
 
 constexpr int kT = 256;
 
-inline int grid_for(int64_t items) {
-  int64_t b = (items + kT - 1) / kT;
-  const int64_t cap = (int64_t)ab_num_sms() * 16;
-  if (b > cap) b = cap;
-  return b < 1 ? 1 : (int)b;
-}
-
 __global__ void __launch_bounds__(kT)
     avgpool_fwd_kernel(const float* __restrict__ x, int ld_x, float* __restrict__ y, int ld_y,
                        int N, int H, int W, int C, int sh, int sw) {
@@ -77,7 +70,7 @@ int atomai_b200_avgpool_fwd(const float* x, int ld_x, float* y, int ld_y, int N,
   AB_CHECK(sh >= 1 && sw >= 1, "avgpool_fwd: window (%d, %d) must be positive", sh, sw);
   const int64_t total = (int64_t)N * (H / sh) * (W / sw) * C;
   if (total == 0) return 0;
-  avgpool_fwd_kernel<<<grid_for(total), kT, 0, STREAM>>>(x, ld_x, y, ld_y, N, H, W, C, sh, sw);
+  avgpool_fwd_kernel<<<ab_grid(total, kT, 16), kT, 0, STREAM>>>(x, ld_x, y, ld_y, N, H, W, C, sh, sw);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -88,7 +81,7 @@ int atomai_b200_upsample_w2x_fwd(const float* x, int ld_x, float* y, int ld_y, i
            "upsample_w2x_fwd: bad arguments");
   const int64_t rows = (int64_t)N * 2 * w;
   if (rows == 0) return 0;
-  upsample_w2x_fwd_kernel<<<grid_for(rows * C), kT, 0, STREAM>>>(x, ld_x, y, ld_y, rows, C);
+  upsample_w2x_fwd_kernel<<<ab_grid(rows * C, kT, 16), kT, 0, STREAM>>>(x, ld_x, y, ld_y, rows, C);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -99,7 +92,7 @@ int atomai_b200_upsample_w2x_bwd(const float* dy, int ld_dy, float* dx, int ld_d
            "upsample_w2x_bwd: bad arguments");
   const int64_t rows = (int64_t)N * w;
   if (rows == 0) return 0;
-  upsample_w2x_bwd_kernel<<<grid_for(rows * C), kT, 0, STREAM>>>(dy, ld_dy, dx, ld_dx, rows, C);
+  upsample_w2x_bwd_kernel<<<ab_grid(rows * C, kT, 16), kT, 0, STREAM>>>(dy, ld_dy, dx, ld_dx, rows, C);
   AB_LAUNCH_CHECK();
   return 0;
 }

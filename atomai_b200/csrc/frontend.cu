@@ -125,12 +125,6 @@ __global__ void __launch_bounds__(kT) rowloss_kernel(const float* __restrict__ x
   }
 }
 
-int grid_for(int64_t n) {
-  int64_t g = (n + kT - 1) / kT;
-  const int64_t cap = (int64_t)ab_num_sms() * 16;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 }  // namespace
 
 extern "C" {
@@ -140,7 +134,7 @@ int atomai_b200_prob_mask(const float* logits, int ld, int64_t npix, int C, int 
   AB_CHECK(logits && prob && C > 0 && ld >= C && ld_p >= C, "prob_mask: bad arguments");
   AB_CHECK(mode >= 0 && mode <= 3, "prob_mask: mode=%d", mode);
   if (npix == 0) return 0;
-  prob_mask_kernel<<<grid_for(npix), kT, 0, (cudaStream_t)stream>>>(logits, ld, npix, C, mode,
+  prob_mask_kernel<<<ab_grid(npix, kT, 16), kT, 0, (cudaStream_t)stream>>>(logits, ld, npix, C, mode,
                                                                      thresh, prob, ld_p, mask);
   AB_LAUNCH_CHECK();
   return 0;
@@ -173,7 +167,7 @@ int atomai_b200_dropout(float* a, int ld, int64_t npix, int C, float p, uint64_t
   AB_CHECK(a && C > 0 && ld >= C && p >= 0.f && p < 1.f, "dropout: bad arguments (p=%f)", p);
   AB_CHECK(C <= 4096, "dropout: too many channels");
   if (npix == 0) return 0;
-  dropout_kernel<<<grid_for(npix * C), kT, 2 * C * sizeof(float), (cudaStream_t)stream>>>(
+  dropout_kernel<<<ab_grid(npix * C, kT, 16), kT, 2 * C * sizeof(float), (cudaStream_t)stream>>>(
       a, ld, npix, C, p, 1.f / (1.f - p), seed, stats);
   AB_LAUNCH_CHECK();
   return 0;

@@ -21,13 +21,6 @@ constexpr int kT = 256;   // 8 warps: 8 pixel rows x 32 channel lanes
 constexpr int kLanes = 32;
 constexpr int kRows = kT / kLanes;
 
-inline int grid_flat(int64_t items) {
-  int64_t b = (items + kT - 1) / kT;
-  const int64_t cap = (int64_t)ab_num_sms() * 16;
-  if (b > cap) b = cap;
-  return b < 1 ? 1 : (int)b;
-}
-
 // CTAs along the pixel axis for a (pixels x channel groups) launch: a function of the shape and the
 // SM count only, so the ordered sums are reproducible
 inline int grid_rows(int64_t rows, int groups) {
@@ -403,7 +396,7 @@ int atomai_b200_dw3x3_dgrad(const float* dy, int ld_dy, const float* w, float* d
   p.dy = dy; p.ld_dy = ld_dy; p.y = dx; p.ld_y = ld_dx;
   const int64_t total = (int64_t)N * H * W * C;
   if (total == 0) return 0;
-  dw_dgrad_kernel<<<grid_flat(total), kT, 0, STREAM>>>(p);
+  dw_dgrad_kernel<<<ab_grid(total, kT, 16), kT, 0, STREAM>>>(p);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -429,7 +422,7 @@ int atomai_b200_affine_relu6(const float* a, int ld_a, const float* scale, const
                              float* y, int ld_y, int64_t npix, int C, void* stream) {
   AB_CHECK(a && scale && shift && y && C > 0 && npix >= 0, "affine_relu6: bad arguments");
   if (npix == 0) return 0;
-  affine_relu6_kernel<<<grid_flat(npix * C), kT, 0, STREAM>>>(a, ld_a, scale, shift, y, ld_y, npix, C);
+  affine_relu6_kernel<<<ab_grid(npix * C, kT, 16), kT, 0, STREAM>>>(a, ld_a, scale, shift, y, ld_y, npix, C);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -439,7 +432,7 @@ int atomai_b200_avgpool_relu6_fwd(const float* a, int ld_a, const float* scale, 
   AB_CHECK(a && y && N >= 0 && HW > 0 && C > 0, "avgpool_relu6_fwd: bad arguments");
   AB_CHECK((scale == nullptr) == (shift == nullptr), "avgpool_relu6_fwd: scale and shift go together");
   if (N == 0) return 0;
-  avgpool_relu6_kernel<<<grid_flat((int64_t)N * C), kT, 0, STREAM>>>(a, ld_a, scale, shift, y, N, HW, C);
+  avgpool_relu6_kernel<<<ab_grid((int64_t)N * C, kT, 16), kT, 0, STREAM>>>(a, ld_a, scale, shift, y, N, HW, C);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -448,7 +441,7 @@ int atomai_b200_avgpool_bwd(const float* dy, float* g, int ld_g, int N, int HW, 
                             void* stream) {
   AB_CHECK(dy && g && N >= 0 && HW > 0 && C > 0 && ld_g >= C, "avgpool_bwd: bad arguments");
   if (N == 0) return 0;
-  avgpool_bwd_kernel<<<grid_flat((int64_t)N * HW * C), kT, 0, STREAM>>>(dy, g, ld_g, N, HW, C);
+  avgpool_bwd_kernel<<<ab_grid((int64_t)N * HW * C, kT, 16), kT, 0, STREAM>>>(dy, g, ld_g, N, HW, C);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -456,7 +449,7 @@ int atomai_b200_avgpool_bwd(const float* dy, float* g, int ld_g, int N, int HW, 
 int atomai_b200_log_softmax_fwd(const float* x, float* y, int B, int C, void* stream) {
   AB_CHECK(x && y && B >= 0 && C > 0, "log_softmax_fwd: bad arguments");
   if (B == 0) return 0;
-  log_softmax_fwd_kernel<<<grid_flat((int64_t)B * 32), kT, 0, STREAM>>>(x, y, B, C);
+  log_softmax_fwd_kernel<<<ab_grid((int64_t)B * 32, kT, 16), kT, 0, STREAM>>>(x, y, B, C);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -465,7 +458,7 @@ int atomai_b200_log_softmax_bwd(const float* y, const float* dy, float* dx, int 
                                 void* stream) {
   AB_CHECK(y && dy && dx && B >= 0 && C > 0, "log_softmax_bwd: bad arguments");
   if (B == 0) return 0;
-  log_softmax_bwd_kernel<<<grid_flat((int64_t)B * 32), kT, 0, STREAM>>>(y, dy, dx, B, C);
+  log_softmax_bwd_kernel<<<ab_grid((int64_t)B * 32, kT, 16), kT, 0, STREAM>>>(y, dy, dx, B, C);
   AB_LAUNCH_CHECK();
   return 0;
 }
@@ -479,7 +472,7 @@ int atomai_b200_nll_fwd_bwd(const float* logp, const int64_t* target, int B, int
     AB_LAUNCH_CHECK();
   }
   if (dlogp) {
-    nll_bwd_kernel<<<grid_flat((int64_t)B * C), kT, 0, STREAM>>>(target, B, C, gscale_dev, dlogp);
+    nll_bwd_kernel<<<ab_grid((int64_t)B * C, kT, 16), kT, 0, STREAM>>>(target, B, C, gscale_dev, dlogp);
     AB_LAUNCH_CHECK();
   }
   return 0;

@@ -12,49 +12,30 @@ namespace {
 
 constexpr int kT = 256;
 
-inline int grid_for(int64_t items) {
-  int64_t b = (items + kT - 1) / kT;
-  const int64_t cap = (int64_t)ab_num_sms() * 16;
-  if (b > cap) b = cap;
-  return b < 1 ? 1 : (int)b;
-}
-
+// W = 4 channels per thread on the float4 path, W = 1 otherwise (common.cuh: Lanes, ChanIdx)
+template <int W>
 __global__ void __launch_bounds__(kT)
     affine_res_act_kernel(const float* __restrict__ a, int ld_a, const float* __restrict__ scale,
                           const float* __restrict__ shift, const float* __restrict__ res,
-                          int ld_res, float slope, float* __restrict__ y, int ld_y, int64_t npix,
-                          int C, int vec) {
-  if (vec) {
-    const int C4 = C >> 2;
-    const int64_t total = npix * C4;
-    for (int64_t i = blockIdx.x * (int64_t)kT + threadIdx.x; i < total; i += (int64_t)gridDim.x * kT) {
-      const int c = (int)(i % C4) * 4;
-      const int64_t pix = i / C4;
-      float4 v = *reinterpret_cast<const float4*>(a + pix * ld_a + c);
-      if (scale) {
-        const float4 s = *reinterpret_cast<const float4*>(scale + c);
-        const float4 t = *reinterpret_cast<const float4*>(shift + c);
-        v.x = fmaf(v.x, s.x, t.x); v.y = fmaf(v.y, s.y, t.y);
-        v.z = fmaf(v.z, s.z, t.z); v.w = fmaf(v.w, s.w, t.w);
-      }
-      if (res) {
-        const float4 r = *reinterpret_cast<const float4*>(res + pix * ld_res + c);
-        v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
-      }
-      v.x = v.x > 0.f ? v.x : v.x * slope; v.y = v.y > 0.f ? v.y : v.y * slope;
-      v.z = v.z > 0.f ? v.z : v.z * slope; v.w = v.w > 0.f ? v.w : v.w * slope;
-      *reinterpret_cast<float4*>(y + pix * ld_y + c) = v;
+                          int ld_res, float slope, float* __restrict__ y, int ld_y,
+                          typename ChanIdx<W>::I total, ChanIdx<W> ix) {
+  using I = typename ChanIdx<W>::I;
+  for (I i = blockIdx.x * (I)kT + threadIdx.x; i < total; i += (I)gridDim.x * kT) {
+    I pix; int c; ix.split(i, pix, c);
+    Lanes<W> v = lanes_ld<W>(a + (size_t)pix * ld_a + c);
+    if (scale) {
+      const Lanes<W> s = lanes_ld<W>(scale + c), t = lanes_ld<W>(shift + c);
+#pragma unroll
+      for (int k = 0; k < W; ++k) v[k] = fmaf(v[k], s[k], t[k]);
     }
-    return;
-  }
-  const int64_t total = npix * C;
-  for (int64_t i = blockIdx.x * (int64_t)kT + threadIdx.x; i < total; i += (int64_t)gridDim.x * kT) {
-    const int c = (int)(i % C);
-    const int64_t pix = i / C;
-    float v = a[pix * ld_a + c];
-    if (scale) v = fmaf(v, scale[c], shift[c]);
-    if (res) v += res[pix * ld_res + c];
-    y[pix * ld_y + c] = v > 0.f ? v : v * slope;
+    if (res) {
+      const Lanes<W> r = lanes_ld<W>(res + (size_t)pix * ld_res + c);
+#pragma unroll
+      for (int k = 0; k < W; ++k) v[k] += r[k];
+    }
+#pragma unroll
+    for (int k = 0; k < W; ++k) v[k] = v[k] > 0.f ? v[k] : v[k] * slope;
+    lanes_at<W>(y + (size_t)pix * ld_y + c) = v;
   }
 }
 
@@ -148,13 +129,14 @@ int atomai_b200_affine_res_act(const float* a, int ld_a, const float* scale, con
   AB_CHECK(a && y && C > 0 && npix >= 0, "affine_res_act: bad arguments");
   AB_CHECK((scale == nullptr) == (shift == nullptr), "affine_res_act: scale and shift go together");
   if (npix == 0) return 0;
-  const auto al = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
-  const int vec = C % 4 == 0 && ld_a % 4 == 0 && ld_y % 4 == 0 && al(a) && al(y) &&
-                  (!scale || (al(scale) && al(shift))) && (!res || (al(res) && ld_res % 4 == 0));
-  affine_res_act_kernel<<<grid_for(npix * C / (vec ? 4 : 1)), kT, 0, STREAM>>>(
-      a, ld_a, scale, shift, res, ld_res, lrelu, y, ld_y, npix, C, vec);
-  AB_LAUNCH_CHECK();
-  return 0;
+  const bool vec = vec_ok(C, {a, y, scale, shift, res}, {ld_a, ld_y, res ? ld_res : 0}, npix * C / 4);
+  return by_width(vec, [&](auto vw) {
+    constexpr int W = decltype(vw)::value;
+    affine_res_act_kernel<W><<<ab_grid(npix * C / W, kT, 16), kT, 0, STREAM>>>(
+        a, ld_a, scale, shift, res, ld_res, lrelu, y, ld_y, npix * C / W, ChanIdx<W>(C));
+    AB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int atomai_b200_lrelu_mask_bwd(const float* dy, int ld_dy, const float* y, int ld_y, float lrelu,
@@ -162,7 +144,7 @@ int atomai_b200_lrelu_mask_bwd(const float* dy, int ld_dy, const float* y, int l
   AB_CHECK(dy && y && g && C > 0 && npix >= 0, "lrelu_mask_bwd: bad arguments");
   AB_CHECK(lrelu > 0.f, "lrelu_mask_bwd: the mask is read from sign(y), which needs slope > 0");
   if (npix == 0) return 0;
-  lrelu_mask_bwd_kernel<<<grid_for(npix * C), kT, 0, STREAM>>>(dy, ld_dy, y, ld_y, lrelu, g, ld_g,
+  lrelu_mask_bwd_kernel<<<ab_grid(npix * C, kT, 16), kT, 0, STREAM>>>(dy, ld_dy, y, ld_y, lrelu, g, ld_g,
                                                               npix, C);
   AB_LAUNCH_CHECK();
   return 0;
@@ -172,7 +154,7 @@ int atomai_b200_resize_fwd(const float* x, int ld_x, float* y, int ld_y, int N, 
                            int factor, int bilinear, void* stream) {
   AB_CHECK(x && y && factor >= 1 && C > 0, "resize_fwd: bad arguments");
   if ((int64_t)N * h * w == 0) return 0;
-  resize_fwd_kernel<<<grid_for((int64_t)N * h * w * factor * factor * C), kT, 0, STREAM>>>(
+  resize_fwd_kernel<<<ab_grid((int64_t)N * h * w * factor * factor * C, kT, 16), kT, 0, STREAM>>>(
       x, ld_x, y, ld_y, N, h, w, C, factor, bilinear);
   AB_LAUNCH_CHECK();
   return 0;
@@ -182,7 +164,7 @@ int atomai_b200_resize_bwd(const float* dy, int ld_dy, float* dx, int ld_dx, int
                            int C, int factor, int bilinear, void* stream) {
   AB_CHECK(dy && dx && factor >= 1 && C > 0, "resize_bwd: bad arguments");
   if ((int64_t)N * h * w == 0) return 0;
-  resize_bwd_kernel<<<grid_for((int64_t)N * h * w * factor * factor * C), kT, 0, STREAM>>>(
+  resize_bwd_kernel<<<ab_grid((int64_t)N * h * w * factor * factor * C, kT, 16), kT, 0, STREAM>>>(
       dy, ld_dy, dx, ld_dx, N, h, w, C, factor, bilinear);
   AB_LAUNCH_CHECK();
   return 0;

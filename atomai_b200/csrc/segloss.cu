@@ -264,12 +264,6 @@ __global__ void iou_finalize_kernel(const int64_t* __restrict__ counts, int nc, 
   *iou = sum / (float)nc;
 }
 
-inline int grid_for(int64_t n) {
-  int64_t g = (n + kT - 1) / kT;
-  const int64_t cap = (int64_t)ab_num_sms() * 8;
-  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 }  // namespace
 
 #define STREAM ((cudaStream_t)stream)
@@ -286,7 +280,7 @@ int atomai_b200_dice_sums(const float* logits, int ld, const void* labels, int l
   Ordered red;
   if (C == 1) {
     const int64_t npix = (int64_t)N * H * W;
-    const int g = grid_for(npix);
+    const int g = ab_grid(npix, kT, 8);
     if (ab_ordered_ws(STREAM, (int64_t)g * 4, 1, &red)) return 1;
     dice_sums_bin_kernel<<<g, kT, 0, STREAM>>>(logits, ld, labels, label_float, npix, cells, red);
     AB_LAUNCH_CHECK();
@@ -329,7 +323,7 @@ int atomai_b200_dice_bwd(const float* logits, int ld, const void* labels, int la
   AB_CHECK(C == 1 || !label_float, "dice_bwd: multi-class labels must be int64");
   const int64_t npix = (int64_t)N * H * W;
   if (npix == 0) return 0;
-  dice_bwd_kernel<<<grid_for(npix), kT, 0, STREAM>>>(logits, ld, labels, label_float, npix, W, C,
+  dice_bwd_kernel<<<ab_grid(npix, kT, 8), kT, 0, STREAM>>>(logits, ld, labels, label_float, npix, W, C,
                                                      coef, dlogits, ld_d, gscale, gscale_dev);
   AB_LAUNCH_CHECK();
   return 0;
@@ -351,7 +345,7 @@ int atomai_b200_iou_hist(const float* logits, int ld, const void* labels, int la
   AB_CHECK(C <= 64, "iou_hist: %d classes (at most 64)", C);
   if (npix == 0) return 0;
   const int nc = C == 1 ? 2 : C;
-  iou_hist_kernel<<<grid_for(npix), kT, nc * nc * sizeof(unsigned), STREAM>>>(
+  iou_hist_kernel<<<ab_grid(npix, kT, 8), kT, nc * nc * sizeof(unsigned), STREAM>>>(
       logits, ld, labels, label_float, npix, C, activation, thresh,
       reinterpret_cast<unsigned long long*>(counts));
   AB_LAUNCH_CHECK();

@@ -6,10 +6,10 @@ Layout control.  Every NHWC operand is placed in a NaN-filled buffer (class Slot
 ld = C + pad and an optional start offset of one float, so each case decides which dispatch path
 runs.  The predicates are mirrored here (vec_ok for elementwise.cu, res_vec_ok for resnet.cu's
 affine_res_act) and each case id names the path it must take ("f4" or "scalar").  The shape grid
-covers C in {1, 3, 5} (scalar only), {12, 24, 48} (float4 with the division branch of VIdx),
+covers C in {1, 3, 5} (scalar only), {12, 24, 48} (float4 with the division branch of ChanIdx<4>),
 {4, 16, 32, 1024} (float4, shift branch), C = 32 with ld = 33 (scalar), odd H and W, h or w = 1
 for the resamplers, N = 1, and launches large enough for the grid-stride loops to go round more
-than once (grid_for caps the grid at 8 x SMs CTAs).
+than once (ab_grid caps the grid at 8 x SMs CTAs in elementwise.cu).
 
 (a) Exact tier.  Small integers, BN scales in +-{0.5, 1, 2}, shifts on a 0.5 grid, LeakyReLU
     slope 0.25, resize factors 2 and 4 and the bilinear x2 weights 1/4 and 3/4: every product and
@@ -27,8 +27,8 @@ than once (grid_for caps the grid at 8 x SMs CTAs).
     0.53 upsample, 0.48 resize, 0.47 log_softmax_bwd, 0.39 bn_finalize, 0.37 bn_act_bwd,
     0.36 linear, 0.22 coord_latent forward, 0.14 gemm, and at most 0.03 for every sum over pixels
     (BatchNorm sums, dbias, losses, coord_latent backward).
-(c) Float4 against scalar.  The float4 and scalar path of every per-element kernel are bitwise
-    identical on the same data (upsample_fwd_blk_kernel included).
+(c) Float4 against scalar.  The W = 4 and W = 1 instances of every per-element kernel are bitwise
+    identical on the same data.
 (d) Sentinels.  Pad channels and the guard floats around each buffer still hold NaN bits after
     every call; every non-accumulating output is NaN-filled first; accumulating outputs start
     from non-zero values.
@@ -36,8 +36,8 @@ than once (grid_for caps the grid at 8 x SMs CTAs).
     atomics of resize_bwd, split-K gemm, the skinny Linear forward and coord_latent_bwd are
     exempt).
 (f) Host-side refusals raise NativeError from argument checks before any launch.
-(g) Dispatch coverage: torch.profiler confirms that both sides of every dual-path entry point
-    were launched.
+(g) Dispatch coverage: torch.profiler confirms that both instances (<4> and <1>) of every dual-path
+    kernel were launched.
 """
 import ctypes as C
 import itertools
@@ -193,11 +193,11 @@ def vec_ok(C, tensors, lds, total4):
 
 
 def res_vec_ok(C, a, y, scale, shift, res):
-    """resnet.cu affine_res_act's `vec` condition."""
-    al = lambda t: t.data_ptr() % 16 == 0
-    return (C % 4 == 0 and ops._ld(a) % 4 == 0 and ops._ld(y) % 4 == 0 and al(a) and al(y) and
-            (scale is None or (al(scale) and al(shift))) and
-            (res is None or (al(res) and ops._ld(res) % 4 == 0)))
+    """resnet.cu affine_res_act's vec_ok call: < 2^31 float4 items, the operands' pointers and
+    pixel strides as in vec_ok."""
+    npix = a.shape[0] * a.shape[1] * a.shape[2]
+    lds = [ops._ld(a), ops._ld(y)] + ([] if res is None else [ops._ld(res)])
+    return vec_ok(C, (a, y, scale, shift, res), lds, npix * C // 4)
 
 
 def exp_vec(C, lay):
@@ -1326,9 +1326,9 @@ def test_dilated_sum_rejects_strided_views(cuda):
 
 # ============================================================================= dispatch coverage
 @gpu
-def test_dispatch_coverage(cuda):
-    """Both sides of every dual-path entry point (and the special kernels) are launched by the
-    cases above; a dispatch rule that changes later shows up here."""
+def test_dispatch_coverage_by_width(cuda):
+    """Both instances (W = 4 and W = 1) of every dual-path kernel (and the special kernels) are
+    launched by the cases above; a dispatch rule that changes later shows up here."""
     from torch.profiler import ProfilerActivity, profile
     dev = cuda
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -1360,11 +1360,12 @@ def test_dispatch_coverage(cuda):
     def launched(pat):
         return any(pat in n for n in names)
 
-    for k in ("affine_vec_kernel", "affine_kernel(", "add_slice_vec_kernel", "add_slice_kernel(",
-              "pool_fwd_vec_kernel", "pool_fwd_kernel(", "pool_bwd_vec_kernel<true>",
-              "pool_bwd_vec_kernel<false>", "pool_bwd_kernel(", "upsample_fwd_blk_kernel",
-              "upsample_fwd_kernel(", "upsample_bwd_vec_kernel", "upsample_bwd_kernel(",
-              "bn_bwd_reduce_vec_kernel", "bn_bwd_reduce_kernel(", "bn_lrelu_bwd_vec_kernel",
-              "bn_lrelu_bwd_kernel(", "affine_res_act_kernel", "skinny_fwd_kernel",
-              "skinny_bwd_kernel<8>", "skinny_bwd_kernel<16>", "gemm_kernel", "bias_fill_kernel"):
+    for k in ("affine_kernel<4>", "affine_kernel<1>", "add_slice_kernel<4>", "add_slice_kernel<1>",
+              "pool_fwd_kernel<4>", "pool_fwd_kernel<1>", "pool_bwd_kernel<4, true>",
+              "pool_bwd_kernel<4, false>", "pool_bwd_kernel<1, false>", "upsample_fwd_kernel<4>",
+              "upsample_fwd_kernel<1>", "upsample_bwd_kernel<4>", "upsample_bwd_kernel<1>",
+              "bn_bwd_reduce_kernel<4>", "bn_bwd_reduce_kernel<1>", "bn_lrelu_bwd_kernel<4>",
+              "bn_lrelu_bwd_kernel<1>", "affine_res_act_kernel<4>", "affine_res_act_kernel<1>",
+              "skinny_fwd_kernel", "skinny_bwd_kernel<8>", "skinny_bwd_kernel<16>", "gemm_kernel",
+              "bias_fill_kernel"):
         assert launched(k), f"{k} was not launched; kernels seen:\n{text}"
