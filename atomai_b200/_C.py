@@ -17,7 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
            "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu",
-           "decomp.cu", "ed_ops.cu", "graph.cu", "coords.cu"]
+           "decomp.cu", "ed_ops.cu", "graph.cu", "coords.cu", "imgen.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -35,6 +35,8 @@ JLAT_ALPHAS = 0
 JLAT_SAMPLE = 1
 GRAPH_MAX_RING = 32     # AB_GRAPH_MAX_RING
 COORDS_MAX_K = 32       # AB_COORDS_MAX_K
+IMGEN_ATOM_INTS = 9     # AB_IMGEN_ATOM_INTS
+IMGEN_FRAME_INTS = 5    # AB_IMGEN_FRAME_INTS
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -190,6 +192,9 @@ SIGNATURES = {
     "atomai_b200_coords_dbscan_labels": (_i, [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_prob_mask": (_i, [_vp, _i, _i64, _i, _i, _f, _vp, _i, _vp, _vp]),
     "atomai_b200_gather_windows": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp]),
+    "atomai_b200_gather_patches": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp]),
+    "atomai_b200_imgen_owner": (_i, [_vp, _i, _vp, _vp, _vp]),
+    "atomai_b200_imgen_fill": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp]),
     "atomai_b200_peak_refine": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_rowloss": (_i, [_vp, _vp, _i, _i64, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_dropout": (_i, [_vp, _i, _i64, _i, _f, C.c_uint64, _vp, _vp]),

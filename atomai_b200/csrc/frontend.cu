@@ -3,8 +3,9 @@
 //   prob_mask       softmax / sigmoid over NHWC logits + thresholded binary mask per class in one
 //                   pass (SegPredictor.forward_ + cv_thresh: atomai/predictors/predictor.py:209-231,
 //                   atomai/utils/img.py:554-564) — the Locator then labels the masks on the host
-//   gather_windows  sub-image extraction around atom coordinates as one gather
-//                   (atomai/utils/img.py:138-180, 298-350) with a per-window NaN flag
+//   gather          sub-image extraction around atom coordinates as one gather
+//                   (atomai/utils/img.py:138-180, 298-350) with a per-window NaN flag, and the
+//                   patches of extract_patches_ (atomai/utils/img.py:353-389) as a bit copy
 //   dropout         in-place inverted dropout from a counter-based hash RNG (nn.Dropout in
 //                   ConvBlock, atomai/nets/blocks.py:68-69) + per-channel sums for BatchNorm / bias
 // All HBM-bound elementwise work: coalesced loads, one pass.
@@ -41,21 +42,27 @@ __global__ void __launch_bounds__(kT) prob_mask_kernel(const float* __restrict__
   }
 }
 
-// one block per window: out[k][i][j][:] = img[frame][sx + i][sy + j][:]
-__global__ void __launch_bounds__(kT) gather_windows_kernel(const float* __restrict__ img, int h,
-                                                             int w, int c,
-                                                             const int32_t* __restrict__ table, int r,
-                                                             float* __restrict__ out,
-                                                             int32_t* __restrict__ nanflag) {
+// one block per window: out[k][i][j][:] = img[origin_k + i * w * c + j * c + :] for a ph x pw
+// window of c channels.  The origin is the element offset offs[k] when given, else it comes from
+// the int32 row {f, sx, sy} of `table`.  T is a float (NaN flag per window) or an unsigned integer
+// of the element's size (a bit copy, no flag).
+template <typename T>
+__global__ void __launch_bounds__(kT) gather_kernel(const T* __restrict__ img, int h, int w, int c,
+                                                    const int32_t* __restrict__ table,
+                                                    const int64_t* __restrict__ offs, int ph, int pw,
+                                                    T* __restrict__ out,
+                                                    int32_t* __restrict__ nanflag) {
   const int k = blockIdx.x;
-  const int f = table[3 * k], sx = table[3 * k + 1], sy = table[3 * k + 2];
-  const int rc = r * c;
-  const float* base = img + (((int64_t)f * h + sx) * w + sy) * c;
-  float* o = out + (int64_t)k * r * rc;
+  const int64_t row = (int64_t)w * c;
+  const T* base = img + (offs ? offs[k]
+                              : ((int64_t)table[3 * k] * h + table[3 * k + 1]) * row +
+                                    (int64_t)table[3 * k + 2] * c);
+  const int pwc = pw * c, n = ph * pwc;
+  T* o = out + (int64_t)k * n;
   int bad = 0;
-  for (int e = threadIdx.x; e < r * rc; e += kT) {
-    const int i = e / rc, jc = e - i * rc;
-    const float v = base[(int64_t)i * w * c + jc];
+  for (int e = threadIdx.x; e < n; e += kT) {
+    const int i = e / pwc, jc = e - i * pwc;
+    const T v = base[i * row + jc];
     o[e] = v;
     bad |= (v != v);
   }
@@ -145,7 +152,39 @@ int atomai_b200_gather_windows(const float* img, int n, int h, int w, int c, con
   AB_CHECK(img && table && out && n > 0 && h > 0 && w > 0 && c > 0 && r > 0 && r <= h && r <= w,
            "gather_windows: bad arguments");
   if (K == 0) return 0;
-  gather_windows_kernel<<<K, kT, 0, (cudaStream_t)stream>>>(img, h, w, c, table, r, out, nanflag);
+  gather_kernel<float><<<K, kT, 0, (cudaStream_t)stream>>>(img, h, w, c, table, nullptr, r, r, out,
+                                                           nanflag);
+  AB_LAUNCH_CHECK();
+  return 0;
+}
+
+int atomai_b200_gather_patches(const void* img, int elem_bytes, int w, int c, const int64_t* offs,
+                               int K, int ph, int pw, void* out, void* stream) {
+  AB_CHECK(img && offs && out && w > 0 && c > 0 && K >= 0 && ph > 0 && pw > 0 && pw <= w &&
+               (int64_t)ph * pw * c <= INT32_MAX,
+           "gather_patches: bad arguments");
+  if (K == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (elem_bytes) {
+    case 1:
+      gather_kernel<uint8_t><<<K, kT, 0, st>>>((const uint8_t*)img, 0, w, c, nullptr, offs, ph, pw,
+                                               (uint8_t*)out, nullptr);
+      break;
+    case 2:
+      gather_kernel<uint16_t><<<K, kT, 0, st>>>((const uint16_t*)img, 0, w, c, nullptr, offs, ph,
+                                                pw, (uint16_t*)out, nullptr);
+      break;
+    case 4:
+      gather_kernel<uint32_t><<<K, kT, 0, st>>>((const uint32_t*)img, 0, w, c, nullptr, offs, ph,
+                                                pw, (uint32_t*)out, nullptr);
+      break;
+    case 8:
+      gather_kernel<unsigned long long><<<K, kT, 0, st>>>((const unsigned long long*)img, 0, w, c,
+                                                          nullptr, offs, ph, pw,
+                                                          (unsigned long long*)out, nullptr);
+      break;
+    default: AB_CHECK(false, "gather_patches: element size %d not in {1, 2, 4, 8}", elem_bytes);
+  }
   AB_LAUNCH_CHECK();
   return 0;
 }

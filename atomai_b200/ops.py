@@ -564,6 +564,29 @@ def gather_windows(img_nhwc, table, r: int, out, nanflag=None) -> None:
                                            ptr(out), ptr(nanflag), stream_ptr()))
 
 
+def gather_patches(img, offs, ph: int, pw: int, out) -> None:
+    """out[k] = the ph x pw window at element offset offs[k] (int64) of a contiguous image whose last
+    two dims are (w, c), as a bit copy; img and out share a dtype of 1, 2, 4 or 8 bytes."""
+    w, c = img.shape[-2:]
+    assert img.is_contiguous() and out.is_contiguous() and img.dtype == out.dtype
+    assert offs.dtype == torch.int64 and offs.is_contiguous() and out.numel() == offs.numel() * ph * pw * c
+    check(lib().atomai_b200_gather_patches(ptr(img), img.element_size(), w, c, ptr(offs),
+                                           offs.shape[0], ph, pw, ptr(out), stream_ptr()))
+
+
+def imgen_masks(atoms, frames, max_pix: int, owner, tpl, out, background: bool) -> None:
+    """Lattice masks: the owner pass over the int32 atom rows, then the fill pass (see
+    include/atomai_b200.h); `owner` must be zeroed, `tpl` and `out` share a dtype."""
+    assert atoms.dtype == owner.dtype == torch.int32 and frames.dtype == torch.int64
+    assert atoms.shape[1:] == (_C.IMGEN_ATOM_INTS,) and frames.shape[1:] == (_C.IMGEN_FRAME_INTS,)
+    assert all(t.is_contiguous() for t in (atoms, frames, owner, tpl, out)) and tpl.dtype == out.dtype
+    check(lib().atomai_b200_imgen_owner(ptr(atoms), atoms.shape[0], ptr(frames), ptr(owner),
+                                        stream_ptr()))
+    check(lib().atomai_b200_imgen_fill(ptr(atoms), ptr(frames), frames.shape[0], max_pix,
+                                       ptr(owner), ptr(tpl), out.element_size(), int(background),
+                                       ptr(out), stream_ptr()))
+
+
 STAT_GMM, STAT_KMEANS, STAT_KPP = 0, 1, 2
 
 

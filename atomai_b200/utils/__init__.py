@@ -4,9 +4,12 @@ from .coords import (cluster_coord, compare_coordinates, find_com, find_coord_cl
                      remove_edge_coord, subimg_trajectories, transform_coordinates)
 from .graphx import (Graph, Node, filter_subgraphs, filter_subgraphs_, find_cycle_clusters,
                      find_cycles, get_interatomic_r, plot_graph)
-from .img import (crop_borders, cv_thresh, extract_random_subimages, extract_subimages,
+from .img import (crop_borders, cv_thresh, extract_patches, extract_patches_,
+                  extract_patches_and_spectra, extract_random_subimages, extract_subimages,
                   extract_subimages_cuda, get_coord_grid,
                   get_imgstack, imcrop_randcoord, imcrop_randpx, img_pad, img_resize)
+from .imgen import (MakeAtom, create_atom_mask_pair, create_lattice_mask,
+                    create_multiclass_lattice_mask, create_multiclass_lattice_mask_)
 from .nn import (average_weights, get_downsample_factor, get_nb_classes, gpu_usage_map,
                  mock_forward, reset_bnorm, sample_weights, set_train_rng, weights_init)
 from .preproc import (array2list, check_image_dims, check_signal_dims, create_batches,

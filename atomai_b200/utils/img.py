@@ -1,8 +1,11 @@
 """
 Image helpers on the prediction path (host-side numpy): padding to the network's downsampling
-factor, binary thresholding and resizing — atomai/utils/img.py:20-40, 112-135, 554-564.
+factor, binary thresholding and resizing — atomai/utils/img.py:20-40, 112-135, 554-564; sub-image
+extraction around atoms, and the random patches and patch / spectrum pairs that make training
+sets (atomai/utils/img.py:138-452), whose crops are gathers on the GPU.
 """
-from typing import Tuple
+from numbers import Integral, Real
+from typing import List, Tuple, Union
 
 import numpy as np
 
@@ -242,3 +245,227 @@ def get_coord_grid(imgdata: np.ndarray, step: int, return_dict: bool = True):
         coord = np.concatenate((coord, np.zeros((coord.shape[0], 1))), axis=-1)
         return {i: coord for i in range(imgdata.shape[0])}
     return np.concatenate([coord for _ in range(imgdata.shape[0])], axis=0)
+
+
+# ------------------------------------------------------------------ bit copies on the device
+# The patch gather and the lattice-mask fill copy elements bit for bit, so any numeric dtype of
+# 1, 2, 4 or 8 bytes runs through one unsigned-integer kernel of that size.  A numpy array is
+# uploaded once and its result copied back; a CUDA tensor stays on its device.
+_BITS_NP = {1: np.uint8, 2: np.int16, 4: np.int32, 8: np.int64}
+
+
+def _is_cuda(a) -> bool:
+    return hasattr(a, "is_cuda") and a.is_cuda
+
+
+def _elem_bytes(dtype) -> int:
+    """element size of a numpy or torch dtype the bit-copy kernels take; TypeError otherwise"""
+    import torch
+    if isinstance(dtype, torch.dtype):
+        size = torch.empty((), dtype=dtype).element_size()
+        ok = not dtype.is_complex or size <= 8
+    else:
+        dtype = np.dtype(dtype)
+        size, ok = dtype.itemsize, dtype.kind in "biufc"
+    if not ok or size not in _BITS_NP:
+        raise TypeError(f"dtype {dtype} is not supported: elements must be numeric and of 1, 2, 4 "
+                        "or 8 bytes")
+    return size
+
+
+def _device_bits(a):
+    """a (numpy or CUDA) as a contiguous CUDA tensor of same-sized integers"""
+    import torch
+    size = _elem_bytes(a.dtype)
+    if _is_cuda(a):
+        return a.contiguous().view({1: torch.uint8, 2: torch.int16, 4: torch.int32,
+                                    8: torch.int64}[size])
+    if not torch.cuda.is_available():
+        raise RuntimeError("this function runs on a CUDA device; none is available")
+    host = torch.from_numpy(np.ascontiguousarray(a).view(_BITS_NP[size]).reshape(np.shape(a)))
+    return host.to("cuda")
+
+
+def _from_bits(t, like):
+    """a device result `t` in the dtype of `like`: a CUDA tensor, or numpy for a numpy `like`"""
+    if _is_cuda(like):
+        return t.view(like.dtype)
+    return t.cpu().numpy().view(like.dtype)
+
+
+# ------------------------------------------------------------------ random patches
+# sklearn.feature_extraction.image.extract_patches_2d, which the reference calls: the same
+# argument checks and errors, patch counts and draws from check_random_state, so the offsets are
+# numpy's; the crops are one gather (atomai_b200_gather_patches) per image stack.
+def _random_state(random_state):
+    if random_state is None or random_state is np.random:
+        return np.random.mtrand._rand
+    if isinstance(random_state, Integral):
+        return np.random.RandomState(random_state)
+    if isinstance(random_state, np.random.RandomState):
+        return random_state
+    raise ValueError(f"{random_state!r} cannot be used to seed a numpy.random.RandomState instance")
+
+
+def _check_max_patches(max_patches) -> None:
+    if max_patches is None:
+        return
+    if isinstance(max_patches, Integral) and not isinstance(max_patches, bool):
+        if max_patches >= 1:
+            return
+    elif isinstance(max_patches, Real) and not isinstance(max_patches, bool) and 0 < max_patches < 1:
+        return
+    raise ValueError("The 'max_patches' parameter must be a float in the range (0, 1), an int in "
+                     f"the range [1, inf) or None. Got {max_patches!r} instead.")
+
+
+def _check_image(image):
+    """sklearn's check_array(allow_nd=True) for the patch source: finite, real, non-empty"""
+    import torch
+    if _is_cuda(image):
+        if image.dtype.is_complex:
+            raise ValueError("Complex data not supported")
+        if image.dtype.is_floating_point and not bool(torch.isfinite(image).all()):
+            raise ValueError("Input contains NaN or infinity.")
+        return
+    if np.iscomplexobj(image):
+        raise ValueError("Complex data not supported")
+    if image.dtype.kind == "f" and not np.isfinite(image).all():
+        raise ValueError("Input contains NaN or infinity.")
+
+
+def _patch_origins(image, patch_size, max_patches, random_state):
+    """(rows, cols) of the patches extract_patches_2d takes from `image`, in its order; the
+    random draws advance `random_state`'s generator as sklearn's do"""
+    _check_max_patches(max_patches)
+    rng = _random_state(random_state)
+    i_h, i_w = image.shape[:2]
+    p_h, p_w = patch_size
+    if p_h > i_h:
+        raise ValueError("Height of the patch should be less than the height of the image.")
+    if p_w > i_w:
+        raise ValueError("Width of the patch should be less than the width of the image.")
+    _check_image(image)
+    n_h, n_w = i_h - p_h + 1, i_w - p_w + 1
+    if not max_patches:
+        ii, jj = np.meshgrid(np.arange(n_h), np.arange(n_w), indexing="ij")
+        return ii.ravel(), jj.ravel()
+    if isinstance(max_patches, Integral):
+        n = min(max_patches, n_h * n_w)
+    else:
+        n = int(max_patches * (n_h * n_w))    # sklearn's rounding: the product first
+    i_s = rng.randint(n_h, size=n)
+    j_s = rng.randint(n_w, size=n)
+    return i_s, j_s
+
+
+def _gather_patches(stack, origins, patch_size):
+    """the patches of every frame of `stack` (f, h, w, ...) at origins [(frame, rows, cols)] as one
+    gather; (K, ph, pw[, c]) in the stack's dtype, numpy or CUDA like the stack"""
+    import torch
+    from .. import ops
+    from .graphx import _check_free
+    ph, pw = patch_size
+    f, h, w = stack.shape[:3]
+    c = int(np.prod(stack.shape[3:], dtype=np.int64))
+    size = _elem_bytes(stack.dtype)
+    K = sum(len(r) for _, r, _ in origins)
+    offs = np.concatenate([(k * h + rows.astype(np.int64)) * w * c + cols.astype(np.int64) * c
+                           for k, rows, cols in origins]) if K else np.zeros(0, np.int64)
+    out_bytes = K * ph * pw * c * size
+    _check_free(out_bytes + (0 if _is_cuda(stack) else f * h * w * c * size) + 8 * K,
+                "the patch gather")
+    img = _device_bits(stack).reshape(f, h, w, c)
+    out = torch.empty((K, ph, pw, c), dtype=img.dtype, device=img.device)
+    if K:
+        ops.gather_patches(img, torch.from_numpy(offs).to(img.device), ph, pw, out)
+    out = _from_bits(out, stack)
+    return out.reshape(K, ph, pw) if c == 1 else out
+
+
+def _extract_pairs(images, masks, patch_size: int, num_patches: int, kwargs):
+    """origins of every frame, images first then masks, then one gather per stack"""
+    rs = kwargs.get("random_state", 0)
+    if isinstance(patch_size, int):
+        patch_size = (patch_size, patch_size)
+    if not isinstance(patch_size, (tuple, list)):
+        raise ValueError("The 'patch_size' parameter must be an instance of 'tuple' or 'list'. "
+                         f"Got {patch_size!r} instead.")
+    im_org, ma_org = [], []
+    for k in range(min(len(images), len(masks))):
+        im_org.append((k, *_patch_origins(images[k], patch_size, num_patches, rs)))
+        ma_org.append((k, *_patch_origins(masks[k], patch_size, num_patches, rs)))
+    if not im_org:
+        raise ValueError("need at least one array to concatenate")
+    return (_gather_patches(images, im_org, patch_size),
+            _gather_patches(masks, ma_org, patch_size))
+
+
+def extract_patches_(lattice_im, lattice_mask, patch_size: int, num_patches: int, **kwargs: int
+                     ) -> Tuple[np.ndarray]:
+    """Patches of `patch_size` (int: square, or (ph, pw)) from an image and its mask, as
+    sklearn's extract_patches_2d takes them with max_patches=num_patches and
+    random_state=kwargs.get('random_state', 0), images drawn first, then masks, from that same
+    argument (atomai/utils/img.py:353-366).  Numpy arrays or CUDA tensors of any numeric dtype of
+    1, 2, 4 or 8 bytes; the crops are one gather on the GPU."""
+    if _is_cuda(lattice_im) is not _is_cuda(lattice_mask):
+        raise TypeError("the image and the mask must both be numpy arrays or both CUDA tensors")
+    if not _is_cuda(lattice_im) and not (isinstance(lattice_im, np.ndarray)
+                                         and isinstance(lattice_mask, np.ndarray)):
+        raise ValueError("The 'image' parameter of extract_patches_2d must be an instance of "
+                         "'numpy.ndarray'")
+    return _extract_pairs(lattice_im[None], lattice_mask[None], patch_size, num_patches, kwargs)
+
+
+def extract_patches(images, masks, patch_size: int, num_patches: int, **kwargs: int
+                    ) -> Tuple[np.ndarray]:
+    """extract_patches_ on every image / mask pair of two stacks with the same arguments, in order,
+    concatenated (atomai/utils/img.py:369-389); a 2-D image or mask is one frame."""
+    if _is_cuda(images) is not _is_cuda(masks):
+        raise TypeError("the images and the masks must both be numpy arrays or both CUDA tensors")
+    if not _is_cuda(images):              # a list of frames, as np.ndim and zip take it
+        images, masks = np.asarray(images), np.asarray(masks)
+    if images.ndim == 2:
+        images = images[None]
+    if masks.ndim == 2:
+        masks = masks[None]
+    return _extract_pairs(images, masks, patch_size, num_patches, kwargs)
+
+
+def extract_patches_and_spectra(hdata: np.ndarray, *args: np.ndarray,
+                                coordinates: np.ndarray = None,
+                                window_size: int = None,
+                                avg_pool: int = 2,
+                                **kwargs: Union[int, List[int]]
+                                ) -> Tuple[np.ndarray]:
+    """Image patches around `coordinates` and the spectra at their centres, from 3-D (h, w, s) or
+    4-D (h, w, s1, s2) hyperspectral data (atomai/utils/img.py:392-452).  The image is args[0] or
+    hdata averaged over kwargs['band'] (an int, or a 2- / 4-element list); patches come from
+    extract_subimages, spectra are hdata[int(x), int(y)] of the kept coordinates, average-pooled
+    over the spectral axes with kernel = stride = avg_pool by torch on the CPU.  Returns
+    (patches, spectra, coordinates), the first two squeezed.  On the host: the spectra are one
+    fancy-indexing gather."""
+    import torch
+    if hdata.ndim not in (3, 4):
+        raise ValueError("Hyperspectral data must 3D or 4D")
+    nspec = hdata.ndim - 2
+    if args:
+        img = args[0]
+        if img.ndim != 2:
+            raise ValueError("Image data must be 2D")
+    else:
+        band = kwargs.get("band", 0)
+        if isinstance(band, int):
+            band = [band, band + 1] * nspec
+        elif nspec == 2 and isinstance(band, list) and len(band) == 2:
+            band = band * 2
+        window = tuple(slice(band[2 * k], band[2 * k + 1]) for k in range(nspec))
+        img = hdata[(Ellipsis,) + window].mean(tuple(range(-nspec, 0)))
+    patches, coords, _ = extract_subimages(img, coordinates, window_size)
+    patches = patches.squeeze()
+    # int() truncates toward zero, and a negative index counts from the end
+    spectra = hdata[coords[:, 0].astype(np.int64), coords[:, 1].astype(np.int64)]
+    pool = torch.nn.functional.avg_pool1d if nspec == 1 else torch.nn.functional.avg_pool2d
+    spectra = torch.from_numpy(np.ascontiguousarray(spectra)).unsqueeze(1)
+    spectra = pool(spectra, avg_pool, avg_pool).squeeze().numpy()
+    return patches, spectra, coords

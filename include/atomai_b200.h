@@ -423,6 +423,29 @@ int atomai_b200_prob_mask(const float* logits, int ld, int64_t npix, int C, int 
  * extraction of atomai/utils/img.py:138-180, 298-350 as one gather. */
 int atomai_b200_gather_windows(const float* img, int n, int h, int w, int c, const int32_t* table,
                                int K, int r, float* out, int32_t* nanflag, void* stream);
+/* out[k] = the ph x pw x c window of a row-major image whose rows hold w * c elements, starting at
+ * element offs[k] (int64, device), for the K windows; a bit copy of elements of elem_bytes in
+ * {1, 2, 4, 8}.  The patches of extract_patches_ (atomai/utils/img.py:353-389), whose offsets
+ * are drawn on the host. */
+int atomai_b200_gather_patches(const void* img, int elem_bytes, int w, int c, const int64_t* offs,
+                               int K, int ph, int pw, void* out, void* stream);
+/* ---- lattice masks of utils.imgen (atomai/utils/imgen.py:82-229) ------------------------------
+ * atoms: K rows of AB_IMGEN_ATOM_INTS int32 {frame, channel, r0, c0, nr, nc, tpl, sr, sc}: the
+ * atom's clamped slice rows r0 .. r0+nr-1, columns c0 .. c0+nc-1, and its template element for
+ * slice pixel (i, j) at tpl + i * sr + j * sc (stride 0 broadcasts).  frames: F rows of
+ * AB_IMGEN_FRAME_INTS int64 {h, w, C, out offset, owner offset}, offsets in elements; the frame's
+ * owner map is C planes of h x w int32 and its output h x w x (C [+ 1]) elements.
+ * imgen_owner: owner[pixel] = max(owner, atom + 1) over each atom's slice (caller zeroes owner).
+ * imgen_fill: every class channel of every pixel = the bits of its owner's template element, or 0;
+ * background = 1: float64, a last channel 1 - sum of the class channels (numpy's pairwise order,
+ * recursive above 128 channels), then every negative value set to 0.  max_pix = the largest h * w. */
+#define AB_IMGEN_ATOM_INTS 9
+#define AB_IMGEN_FRAME_INTS 5
+int atomai_b200_imgen_owner(const int32_t* atoms, int K, const int64_t* frames, int32_t* owner,
+                            void* stream);
+int atomai_b200_imgen_fill(const int32_t* atoms, const int64_t* frames, int F, int64_t max_pix,
+                           const int32_t* owner, const void* tpl, int elem_bytes, int background,
+                           void* out, void* stream);
 /* 2-D Gaussian peak refinement (atomai/utils/coords.py:152-231, predictors/predictor.py:609-619):
  * for each of the K rows {frame, row0, col0, d} of `atoms` (int32, device) one least-squares fit of
  *   offset + amp exp(-(a (x-xo)^2 + 2 b (x-xo)(y-yo) + c (y-yo)^2))
