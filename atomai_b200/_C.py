@@ -17,7 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
            "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu",
-           "decomp.cu", "ed_ops.cu", "graph.cu", "coords.cu", "imgen.cu"]
+           "decomp.cu", "ed_ops.cu", "graph.cu", "coords.cu", "imgen.cu", "blobs.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -37,6 +37,7 @@ GRAPH_MAX_RING = 32     # AB_GRAPH_MAX_RING
 COORDS_MAX_K = 32       # AB_COORDS_MAX_K
 IMGEN_ATOM_INTS = 9     # AB_IMGEN_ATOM_INTS
 IMGEN_FRAME_INTS = 5    # AB_IMGEN_FRAME_INTS
+BLOB_U8, BLOB_I16, BLOB_U16, BLOB_F32, BLOB_F64, BLOB_I32 = range(6)   # AB_BLOB_*
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -195,6 +196,7 @@ SIGNATURES = {
     "atomai_b200_gather_patches": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _vp]),
     "atomai_b200_imgen_owner": (_i, [_vp, _i, _vp, _vp, _vp]),
     "atomai_b200_imgen_fill": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp]),
+    "atomai_b200_blob_filter": (_i, [_vp, _i, _i64, _i, _i, _d, _d, _i, _vp, _vp, _vp, _i, _vp]),
     "atomai_b200_peak_refine": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_rowloss": (_i, [_vp, _vp, _i, _i64, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_dropout": (_i, [_vp, _i, _i64, _i, _f, C.c_uint64, _vp, _vp]),

@@ -587,6 +587,25 @@ def imgen_masks(atoms, frames, max_pix: int, owner, tpl, out, background: bool) 
                                        ptr(out), stream_ptr()))
 
 
+BLOB_CODES = {torch.uint8: _C.BLOB_U8, torch.int16: _C.BLOB_I16, torch.uint16: _C.BLOB_U16,
+              torch.float32: _C.BLOB_F32, torch.float64: _C.BLOB_F64, torch.int32: _C.BLOB_I32}
+
+
+def blob_filter(img, im_thresh: float, blob_thresh: float, above: bool, labels, counts,
+                out) -> None:
+    """Threshold, 4-connected labelling and size filter of every frame of the (n, h, w) stack
+    `img` into `out` (see include/atomai_b200.h); `labels` and `counts` are (n, h, w) int32
+    workspaces, left holding each pixel's smallest component index and the component sizes."""
+    assert img.dim() == 3 and img.dtype in BLOB_CODES and img.dtype != torch.int32
+    assert labels.dtype == counts.dtype == torch.int32 and out.dtype in BLOB_CODES
+    assert labels.shape == counts.shape == out.shape == img.shape
+    assert all(t.is_contiguous() for t in (img, labels, counts, out))
+    n, h, w = img.shape
+    check(lib().atomai_b200_blob_filter(ptr(img), BLOB_CODES[img.dtype], n, h, w, im_thresh,
+                                        blob_thresh, int(above), ptr(labels), ptr(counts),
+                                        ptr(out), BLOB_CODES[out.dtype], stream_ptr()))
+
+
 STAT_GMM, STAT_KMEANS, STAT_KPP = 0, 1, 2
 
 

@@ -6,7 +6,7 @@ from .graphx import (Graph, Node, filter_subgraphs, filter_subgraphs_, find_cycl
                      find_cycles, get_interatomic_r, plot_graph)
 from .img import (crop_borders, cv_thresh, extract_patches, extract_patches_,
                   extract_patches_and_spectra, extract_random_subimages, extract_subimages,
-                  extract_subimages_cuda, get_coord_grid,
+                  extract_subimages_cuda, filter_cells, filter_cells_, get_coord_grid,
                   get_imgstack, imcrop_randcoord, imcrop_randpx, img_pad, img_resize)
 from .imgen import (MakeAtom, create_atom_mask_pair, create_lattice_mask,
                     create_multiclass_lattice_mask, create_multiclass_lattice_mask_)

@@ -2,7 +2,8 @@
 Image helpers on the prediction path (host-side numpy): padding to the network's downsampling
 factor, binary thresholding and resizing — atomai/utils/img.py:20-40, 112-135, 554-564; sub-image
 extraction around atoms, and the random patches and patch / spectrum pairs that make training
-sets (atomai/utils/img.py:138-452), whose crops are gathers on the GPU.
+sets (atomai/utils/img.py:138-452), whose crops are gathers on the GPU; the blob-size filter of
+segmented frames (atomai/utils/img.py:567-625), labelled on the GPU.
 """
 from numbers import Integral, Real
 from typing import List, Tuple, Union
@@ -27,6 +28,95 @@ def cv_thresh(imgdata: np.ndarray, threshold: float = .5) -> np.ndarray:
     """cv2.threshold(img, threshold, 1, THRESH_BINARY): 1.0 where img > threshold else 0.0, same
     dtype as the input (atomai/utils/img.py:554-564).  Pure numpy so cv2 is not a dependency."""
     return (imgdata > threshold).astype(imgdata.dtype)
+
+
+# ------------------------------------------------------------------ blob filtering
+# atomai/utils/img.py:567-625 runs cv2.threshold, scipy.ndimage.label (4-connectivity) and
+# ndimage.sum frame by frame.  Here the threshold, the labelling and the size test of every frame
+# of a stack run in csrc/blobs.cu; the host only checks the arguments.
+_BLOB_NP = tuple(np.dtype(t) for t in (np.uint8, np.int16, np.uint16, np.float32, np.float64))
+
+
+def _blob_check(imgdata, ndim: int, im_thresh, blob_thresh, filter_) -> bool:
+    """the argument checks of filter_cells[_], all before any device work; returns `above`"""
+    import torch
+    if _is_cuda(imgdata):
+        ok = imgdata.dtype in (torch.uint8, torch.int16, torch.uint16, torch.float32, torch.float64)
+    elif isinstance(imgdata, np.ndarray):
+        ok = imgdata.dtype in _BLOB_NP
+    else:
+        raise TypeError(f"imgdata must be a numpy array or a CUDA tensor, not {type(imgdata)}")
+    if imgdata.ndim != ndim:
+        raise ValueError(f"imgdata must be {ndim}-D, got shape {tuple(imgdata.shape)}")
+    if not ok:
+        raise TypeError(f"dtype {imgdata.dtype} is not supported: cv2.threshold takes uint8, int16, "
+                        "uint16, float32 and float64")
+    for name, v in (("im_thresh", im_thresh), ("blob_thresh", blob_thresh)):
+        if not isinstance(v, Real):
+            raise TypeError(f"{name} must be a real number, not {type(v)}")
+    if not np.isfinite(float(im_thresh)):
+        raise ValueError(f"im_thresh must be finite, got {im_thresh}")
+    h, w = imgdata.shape[-2:]
+    if h * w >= 2**31:
+        raise ValueError(f"frames of {h} x {w} pixels are too large: at most 2^31 - 1 pixels")
+    if (ndim == 2 or imgdata.shape[0]) and not h * w:
+        raise TypeError("cv2.threshold returns no image for an empty frame")
+    return bool(filter_ == 'above')
+
+
+def _filter_blobs(stack, im_thresh, blob_thresh, above: bool, out_dtype):
+    """the kept-blob mask of every frame of an (n, h, w) stack, numpy or CUDA like the stack"""
+    import torch
+    from .. import ops
+    from .graphx import _check_free
+    cuda = _is_cuda(stack)
+    if 0 in tuple(stack.shape):
+        if cuda:
+            return torch.zeros(stack.shape, dtype=out_dtype, device=stack.device)
+        return np.zeros(stack.shape, out_dtype)
+    if not cuda:
+        out_dtype = torch.from_numpy(np.zeros(0, out_dtype)).dtype
+    npix = int(np.prod(stack.shape, dtype=np.int64))
+    in_bytes = stack.element_size() if cuda else stack.itemsize
+    out_bytes = torch.empty((), dtype=out_dtype).element_size()
+    _check_free(npix * (8 + out_bytes + (0 if cuda else in_bytes)), "the blob filter")
+    if cuda:
+        img = stack.contiguous()
+    else:
+        if not torch.cuda.is_available():
+            raise RuntimeError("this function runs on a CUDA device; none is available")
+        img = torch.from_numpy(np.ascontiguousarray(stack)).to("cuda")
+    labels = torch.empty(img.shape, dtype=torch.int32, device=img.device)
+    counts = torch.empty_like(labels)
+    out = torch.empty(img.shape, dtype=out_dtype, device=img.device)
+    ops.blob_filter(img, float(im_thresh), float(blob_thresh), above, labels, counts, out)
+    return out if cuda else out.cpu().numpy()
+
+
+def filter_cells_(imgdata: np.ndarray,
+                  im_thresh: float = .5,
+                  blob_thresh: int = 150,
+                  filter_: str = 'below') -> np.ndarray:
+    """Removes the blobs of one (h, w) frame that are smaller than `blob_thresh` pixels (or, with
+    filter_='above', larger), after thresholding at `im_thresh` (atomai/utils/img.py:567-584).
+    Blobs are 4-connected; the result is an int32 0/1 (h, w) array, or a CUDA tensor for a CUDA
+    input.  Input dtypes are cv2.threshold's: uint8, int16, uint16, float32 and float64."""
+    import torch
+    above = _blob_check(imgdata, 2, im_thresh, blob_thresh, filter_)
+    out = _filter_blobs(imgdata[None], im_thresh, blob_thresh, above,
+                        torch.int32 if _is_cuda(imgdata) else np.int32)
+    return out[0]
+
+
+def filter_cells(imgdata: np.ndarray,
+                 im_thresh: float = 0.5,
+                 blob_thresh: int = 50,
+                 filter_: str = 'below') -> np.ndarray:
+    """filter_cells_ on every frame of an (n, h, w) stack (atomai/utils/img.py:598-625); the
+    result has the input's shape and dtype, 1 on the kept blobs.  All frames run in one pass of
+    each GPU kernel."""
+    above = _blob_check(imgdata, 3, im_thresh, blob_thresh, filter_)
+    return _filter_blobs(imgdata, im_thresh, blob_thresh, above, imgdata.dtype)
 
 
 def img_resize(image_data: np.ndarray, rs: Tuple[int], round_: bool = False) -> np.ndarray:

@@ -446,6 +446,25 @@ int atomai_b200_imgen_owner(const int32_t* atoms, int K, const int64_t* frames, 
 int atomai_b200_imgen_fill(const int32_t* atoms, const int64_t* frames, int F, int64_t max_pix,
                            const int32_t* owner, const void* tpl, int elem_bytes, int background,
                            void* out, void* stream);
+/* ---- blob filtering of utils.filter_cells[_] (atomai/utils/img.py:567-625) --------------------
+ * For every frame of the row-major (n, h, w) stack `img` (h * w < 2^31): a pixel is foreground
+ * when img > im_thresh (float32 pixels against (float)im_thresh, the others in double; NaN is
+ * background); the 4-connected components of the foreground are labelled; a component is dropped
+ * when its pixel count c has c > blob_thresh (above != 0) or c < blob_thresh (above == 0), compared
+ * in double, so a NaN blob_thresh keeps every component; out = 1 on the pixels of kept components,
+ * 0 elsewhere, in out_dtype.  Frames never join.  labels and counts are caller-owned n * h * w int32
+ * workspaces, overwritten: afterwards labels[pixel] is the smallest frame-local linear index of the
+ * pixel's component (-1 on the background) and counts[root] the component's size at that index.
+ * dtype: AB_BLOB_U8 .. AB_BLOB_F64; out_dtype: any AB_BLOB_* code.  All passes run on `stream`. */
+#define AB_BLOB_U8 0
+#define AB_BLOB_I16 1
+#define AB_BLOB_U16 2
+#define AB_BLOB_F32 3
+#define AB_BLOB_F64 4
+#define AB_BLOB_I32 5
+int atomai_b200_blob_filter(const void* img, int dtype, int64_t n, int h, int w, double im_thresh,
+                            double blob_thresh, int above, int32_t* labels, int32_t* counts,
+                            void* out, int out_dtype, void* stream);
 /* 2-D Gaussian peak refinement (atomai/utils/coords.py:152-231, predictors/predictor.py:609-619):
  * for each of the K rows {frame, row0, col0, d} of `atoms` (int32, device) one least-squares fit of
  *   offset + amp exp(-(a (x-xo)^2 + 2 b (x-xo)(y-yo) + c (y-yo)^2))
