@@ -95,7 +95,8 @@ __global__ void __launch_bounds__(kT) dropout_kernel(float* __restrict__ a, int 
 
 // per-sample reconstruction loss of the VAEs (atomai/losses_metrics/vi_losses.py:13-37):
 // kind 0: out[b] = 0.5 * sum_j (xhat - x)^2 ; kind 1: sum_j BCE-with-logits(xhat, x).
-// grid = (chunks, B); float4 loads when D % 4 == 0; one double atomic per block.
+// grid = (chunks, B), scalar loads; one double atomic per block, so out is not bitwise
+// reproducible when a row has more than one chunk.
 // dxhat (nullable) = gvec[b] * dloss/dxhat.
 __global__ void __launch_bounds__(kT) rowloss_kernel(const float* __restrict__ x,
                                                       const float* __restrict__ xhat, int64_t D,

@@ -272,11 +272,16 @@ extern "C" {
 
 int atomai_b200_dice_sums(const float* logits, int ld, const void* labels, int label_float, int N,
                           int H, int W, int C, double* cells, void* stream) {
-  AB_CHECK(logits && labels && cells && N >= 0 && H > 0 && W > 0 && C >= 1 && ld >= C,
+  // an empty batch has no logits or labels to point at (torch gives empty tensors a null pointer)
+  AB_CHECK(cells && N >= 0 && H > 0 && W > 0 && C >= 1 && ld >= C && (N == 0 || (logits && labels)),
            "dice_sums: bad arguments");
   AB_CHECK(C <= 16, "dice_sums: %d classes (at most 16)", C);
   AB_CHECK(C == 1 || !label_float, "dice_sums: multi-class labels must be int64");
-  if (N == 0) return 0;
+  if (N == 0) {  // every sum is empty: the cells are zero and the loss is 1 - mean(0 / eps) = 1
+    const int64_t K = C == 1 ? 2 : (int64_t)C * W;
+    AB_CUDA(cudaMemsetAsync(cells, 0, 2 * K * sizeof(double), STREAM));
+    return 0;
+  }
   Ordered red;
   if (C == 1) {
     const int64_t npix = (int64_t)N * H * W;
@@ -317,8 +322,8 @@ int atomai_b200_dice_finalize(const double* cells, int K, float eps, float* loss
 int atomai_b200_dice_bwd(const float* logits, int ld, const void* labels, int label_float, int N,
                          int H, int W, int C, const float* coef, float* dlogits, int ld_d,
                          float gscale, const float* gscale_dev, void* stream) {
-  AB_CHECK(logits && labels && coef && dlogits && N >= 0 && H > 0 && W > 0 && C >= 1 && ld >= C &&
-               ld_d >= C,
+  AB_CHECK(coef && N >= 0 && H > 0 && W > 0 && C >= 1 && ld >= C && ld_d >= C &&
+               (N == 0 || (logits && labels && dlogits)),
            "dice_bwd: bad arguments");
   AB_CHECK(C == 1 || !label_float, "dice_bwd: multi-class labels must be int64");
   const int64_t npix = (int64_t)N * H * W;

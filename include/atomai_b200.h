@@ -261,7 +261,7 @@ int atomai_b200_pointwise_loss(const float* pred, const float* target, int64_t n
  * there are K = C*W cells (class, image column).  C == 1: probabilities [sigmoid, 1 - sigmoid],
  * targets [y == 1, y == 0] of (N, 1, H, W) labels (float if label_float, else int64), K = 2.
  * dice_sums writes cells[0:K] = I = sum p*t and cells[K:2K] = S = sum (p + t) (double, ordered
- * cross-CTA sums, C <= 16, 2*C*ceil(W/32)*32 <= 2^21).  dice_finalize: loss[0] = 1 - mean 2I/(S+eps)
+ * cross-CTA sums, C <= 16, 2*C*ceil(W/32)*32 <= 2^21; N = 0 zeroes them).  dice_finalize: loss[0] = 1 - mean 2I/(S+eps)
  * and coef[0:K] = -(2/K)/(S+eps), coef[K:2K] = (2/K) I/(S+eps)^2 (nullable).  dice_bwd:
  * dlogits = g * dL/dlogits with dL/dp = t*coef[k] + coef[K+k], chained through the softmax /
  * sigmoid, g = gscale * (gscale_dev ? *gscale_dev : 1). */

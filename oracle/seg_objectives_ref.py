@@ -31,6 +31,14 @@ def dice_loss(logits: torch.Tensor, labels: torch.Tensor, eps: float = 1e-7) -> 
     return 1 - (2.0 * inter / (card + eps)).mean()
 
 
+def dice_coefficients(inter: torch.Tensor, card: torch.Tensor, eps: float = 1e-7):
+    """(A, B) with dL/dp = t A + B of the dice loss for each cell's probability p and target t:
+    A = dL/dI = -(2/K) / (S + eps), B = dL/dS = (2/K) I / (S + eps)^2, K cells."""
+    K = inter.numel()
+    d = card + eps
+    return -(2.0 / K) / d, (2.0 / K) * inter / (d * d)
+
+
 def focal_loss(logits: torch.Tensor, target: torch.Tensor, alpha: float = 0.5,
                gamma: float = 2.0) -> torch.Tensor:
     """alpha (1 - pt)^gamma CE, CE = mean BCE-with-logits, pt = exp(-CE)."""
@@ -39,17 +47,28 @@ def focal_loss(logits: torch.Tensor, target: torch.Tensor, alpha: float = 0.5,
     return alpha * (1 - pt) ** gamma * ce
 
 
-def iou_counts(true: torch.Tensor, logits: torch.Tensor, thresh: float = 0.5) -> torch.Tensor:
-    """(nc, nc) int64 confusion histogram (rows true, columns predicted) of the reference's IoU
-    with activation: predicted class = sum_c c [p_c > thresh], 0 above C - 1; C == 1 -> two
-    classes, [sigmoid > thresh]; labels outside [0, nc) skipped."""
+def focal_factor(ce: torch.Tensor, alpha: float = 0.5, gamma: float = 2.0) -> torch.Tensor:
+    """dfocal/dCE = alpha [(1 - pt)^gamma + gamma pt (1 - pt)^(gamma - 1) CE]; the second term is
+    dropped for gamma == 0, as autograd does (it is NaN at CE = 0 for 0 < gamma < 1, as there)."""
+    pt = torch.exp(-ce)
+    q = 1 - pt
+    tail = gamma * pt * q ** (gamma - 1) * ce if gamma != 0 else torch.zeros_like(ce)
+    return alpha * (q ** gamma + tail)
+
+
+def iou_counts(true: torch.Tensor, logits: torch.Tensor, thresh: float = 0.5,
+               activation: bool = True) -> torch.Tensor:
+    """(nc, nc) int64 confusion histogram (rows true, columns predicted) of the reference's IoU:
+    predicted class = sum_c c [p_c > thresh], 0 above C - 1; C == 1 -> two classes,
+    [sigmoid > thresh]; p = softmax / sigmoid, or the raw values without `activation`; labels
+    outside [0, nc) skipped."""
     C = logits.shape[1]
     if C == 1:
         nc = 2
-        pred = (torch.sigmoid(logits[:, 0]) > thresh).long()
+        pred = ((torch.sigmoid(logits[:, 0]) if activation else logits[:, 0]) > thresh).long()
     else:
         nc = C
-        m = (torch.softmax(logits, 1) > thresh).long()
+        m = ((torch.softmax(logits, 1) if activation else logits) > thresh).long()
         cls = torch.arange(C, device=logits.device).reshape(1, C, 1, 1)
         pred = (m * cls).sum(1)
         pred[pred > C - 1] = 0

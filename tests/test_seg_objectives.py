@@ -1,6 +1,7 @@
 """CPU checks of the segmentation objectives: the torch restatement (oracle/seg_objectives_ref.py)
 against the unmodified reference's outputs (tests/golden/seg_objectives.npz), the reference's
 module names, the CUDA-only contract, and the kernels' register budgets."""
+import math
 import os
 import re
 import subprocess
@@ -55,6 +56,55 @@ def test_oracle_focal_matches_reference(gold):
     np.testing.assert_allclose(loss, gold["bin_32x32/focal_loss"], rtol=1e-6)
     np.testing.assert_allclose(g, gold["bin_32x32/focal_grad"], rtol=1e-6,
                                atol=1e-6 * np.abs(gold["bin_32x32/focal_grad"]).max())
+
+
+@pytest.mark.parametrize("name", list(sc.CASES))
+def test_oracle_dice_coefficients_match_autograd(name):
+    """dice_finalize's (A, B), chained through the softmax / sigmoid as dice_bwd does, give the
+    float64 autograd gradient of the oracle's dice_loss."""
+    x, y = sc.case(name)
+    x = torch.from_numpy(x).double().requires_grad_(True)
+    y = torch.from_numpy(y)
+    yy = y.double() if x.shape[1] == 1 else y
+    ref.dice_loss(x, yy).backward()
+    inter, card = ref.dice_cells(x.detach(), yy)
+    A, B = ref.dice_coefficients(inter, card)
+    N, C, H, W = x.shape
+    if C == 1:
+        yl = y[:, 0].long()
+        s = torch.sigmoid(x.detach()[:, 0])
+        G0 = (yl == 1).double() * A[0] + B[0]
+        G1 = (yl == 0).double() * A[1] + B[1]
+        g = (s * (1 - s) * (G0 - G1))[:, None]
+    else:
+        p = torch.softmax(x.detach(), 1)
+        t = torch.nn.functional.one_hot(y, C).permute(0, 3, 1, 2).double()
+        G = t * A.reshape(1, C, 1, W) + B.reshape(1, C, 1, W)
+        g = p * (G - (p * G).sum(1, keepdim=True))
+    err = float((g - x.grad).abs().max() / x.grad.abs().max())
+    assert err <= 1e-13, err
+
+
+@pytest.mark.parametrize("gamma", [0.0, 0.5, 1.0, 2.0, 3.7])
+@pytest.mark.parametrize("alpha", [0.25, 1.0])
+def test_oracle_focal_factor_matches_autograd(alpha, gamma):
+    """focal_factor is dfocal/dCE: the oracle's focal_loss gradient over the BCE gradient."""
+    for ce in (1e-8, 1e-3, 0.3, 1.0, 7.5, 50.0):
+        x = torch.tensor([math.log(math.expm1(ce))], dtype=torch.float64, requires_grad=True)
+        t = torch.zeros(1, dtype=torch.float64)
+        ref.focal_loss(x, t, alpha, gamma).backward()
+        ce64 = torch.nn.functional.binary_cross_entropy_with_logits(x.detach(), t)
+        want = float(x.grad) / float(torch.sigmoid(x.detach()))    # dCE/dx = sigmoid(x) at t = 0
+        got = float(ref.focal_factor(ce64, alpha, gamma))
+        assert abs(got - want) <= 1e-12 * abs(want) + 1e-300, (ce, got, want)
+    # CE = 0: autograd's 0 * inf for 0 < gamma < 1 is NaN, and focal_factor says so too
+    x = torch.tensor([-1000.0], dtype=torch.float64, requires_grad=True)
+    ref.focal_loss(x, torch.zeros(1, dtype=torch.float64), alpha, gamma).backward()
+    ce = torch.zeros((), dtype=torch.float64, requires_grad=True)
+    (alpha * (1 - torch.exp(-ce)) ** gamma * ce).backward()
+    got = ref.focal_factor(torch.zeros((), dtype=torch.float64), alpha, gamma)
+    assert torch.equal(got, ce.grad) or (bool(got.isnan()) and bool(ce.grad.isnan()))
+    assert bool(x.grad.isnan()) == (0 < gamma < 1)
 
 
 @pytest.mark.parametrize("name", list(sc.CASES))
