@@ -17,7 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "conv_tc.cu", "conv_simt.cu", "wgrad_tc.cu", "elementwise.cu",
            "selftest_tma.cu", "vae.cu", "gram.cu", "frontend.cu", "augment.cu", "p2p.cu", "resnet.cu",
            "segloss.cu", "refine.cu", "jlatent.cu", "mobilenet.cu", "gpr.cu", "stat.cu",
-           "decomp.cu", "ed_ops.cu", "graph.cu", "coords.cu", "imgen.cu", "blobs.cu"]
+           "decomp.cu", "ed_ops.cu", "graph.cu", "coords.cu", "imgen.cu", "blobs.cu", "fft.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -38,6 +38,9 @@ COORDS_MAX_K = 32       # AB_COORDS_MAX_K
 IMGEN_ATOM_INTS = 9     # AB_IMGEN_ATOM_INTS
 IMGEN_FRAME_INTS = 5    # AB_IMGEN_FRAME_INTS
 BLOB_U8, BLOB_I16, BLOB_U16, BLOB_F32, BLOB_F64, BLOB_I32 = range(6)   # AB_BLOB_*
+(FFT_U8, FFT_I8, FFT_I16, FFT_U16, FFT_I32, FFT_U32, FFT_I64, FFT_U64, FFT_F16, FFT_F32, FFT_F64,
+ FFT_C64, FFT_C128) = range(13)                                        # AB_FFT_*
+FFT_MAX_SIDE, FFT_MAX_POW2 = 4096, 8192                                # AB_FFT_MAX_*
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -197,6 +200,9 @@ SIGNATURES = {
     "atomai_b200_imgen_owner": (_i, [_vp, _i, _vp, _vp, _vp]),
     "atomai_b200_imgen_fill": (_i, [_vp, _vp, _i, _i64, _vp, _vp, _i, _i, _vp, _vp]),
     "atomai_b200_blob_filter": (_i, [_vp, _i, _i64, _i, _i, _d, _d, _i, _vp, _vp, _vp, _i, _vp]),
+    "atomai_b200_fft2_workspace_bytes": (_i64, [_i, _i]),
+    "atomai_b200_fft2_mask": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _i64, _vp]),
+    "atomai_b200_fft2_sub": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _i, _vp, _i64, _vp]),
     "atomai_b200_peak_refine": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_rowloss": (_i, [_vp, _vp, _i, _i64, _i, _vp, _vp, _vp, _vp]),
     "atomai_b200_dropout": (_i, [_vp, _i, _i64, _i, _f, C.c_uint64, _vp, _vp]),

@@ -606,6 +606,52 @@ def blob_filter(img, im_thresh: float, blob_thresh: float, above: bool, labels, 
                                         ptr(out), BLOB_CODES[out.dtype], stream_ptr()))
 
 
+FFT_CODES = {torch.uint8: _C.FFT_U8, torch.bool: _C.FFT_U8, torch.int8: _C.FFT_I8,
+             torch.int16: _C.FFT_I16, torch.uint16: _C.FFT_U16, torch.int32: _C.FFT_I32,
+             torch.uint32: _C.FFT_U32, torch.int64: _C.FFT_I64, torch.uint64: _C.FFT_U64,
+             torch.float16: _C.FFT_F16, torch.float32: _C.FFT_F32, torch.float64: _C.FFT_F64,
+             torch.complex64: _C.FFT_C64, torch.complex128: _C.FFT_C128}
+
+
+def fft2_workspace_bytes(h: int, w: int) -> int:
+    """bytes of device scratch fft2_mask / fft2_sub need for an (h, w) array (-1: side too long)"""
+    return int(lib().atomai_b200_fft2_workspace_bytes(h, w))
+
+
+def _fft2_work(h: int, w: int):
+    n = fft2_workspace_bytes(h, w)
+    assert n > 0, (h, w)
+    return torch.empty(n, dtype=torch.uint8, device="cuda"), n
+
+
+def fft2_mask(img, r0: int, c0: int, l: int, f2, f3) -> None:
+    """f2 = fftshift(fft2(img)) and f3 = f2 with the disk of half-width l at (r0, c0) zeroed, both
+    (h, w) complex64 or complex128, from a float64 transform (see include/atomai_b200.h)"""
+    assert img.dim() == 2 and img.dtype in FFT_CODES and img.is_contiguous()
+    assert f2.dtype == f3.dtype and f2.dtype in (torch.complex64, torch.complex128)
+    assert f2.shape == f3.shape == img.shape and f2.is_contiguous() and f3.is_contiguous()
+    h, w = img.shape
+    work, nbytes = _fft2_work(h, w)
+    check(lib().atomai_b200_fft2_mask(ptr(img), FFT_CODES[img.dtype], h, w, r0, c0, l, ptr(f2),
+                                      ptr(f3), int(f2.dtype == torch.complex64), ptr(work),
+                                      nbytes, stream_ptr()))
+
+
+def fft2_sub(img, spec, out) -> None:
+    """out = min-max normalised |img - Re(ifft2(ifftshift(spec)))|, float32 or float64, computed
+    in float64 (see include/atomai_b200.h)"""
+    assert img.dim() == 2 and img.dtype in FFT_CODES and img.is_contiguous()
+    assert spec.dtype in (torch.complex64, torch.complex128) and spec.is_contiguous()
+    assert out.dtype in (torch.float32, torch.float64) and out.is_contiguous()
+    assert spec.shape == out.shape == img.shape
+    h, w = img.shape
+    work, nbytes = _fft2_work(h, w)
+    check(lib().atomai_b200_fft2_sub(ptr(img), FFT_CODES[img.dtype], ptr(spec),
+                                     FFT_CODES[spec.dtype], h, w, ptr(out),
+                                     int(out.dtype == torch.float32), ptr(work), nbytes,
+                                     stream_ptr()))
+
+
 STAT_GMM, STAT_KMEANS, STAT_KPP = 0, 1, 2
 
 

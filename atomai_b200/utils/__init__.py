@@ -4,10 +4,10 @@ from .coords import (cluster_coord, compare_coordinates, find_com, find_coord_cl
                      remove_edge_coord, subimg_trajectories, transform_coordinates)
 from .graphx import (Graph, Node, filter_subgraphs, filter_subgraphs_, find_cycle_clusters,
                      find_cycles, get_interatomic_r, plot_graph)
-from .img import (crop_borders, cv_thresh, extract_patches, extract_patches_,
+from .img import (FFTmask, FFTsub, crop_borders, cv_thresh, extract_patches, extract_patches_,
                   extract_patches_and_spectra, extract_random_subimages, extract_subimages,
                   extract_subimages_cuda, filter_cells, filter_cells_, get_coord_grid,
-                  get_imgstack, imcrop_randcoord, imcrop_randpx, img_pad, img_resize)
+                  get_imgstack, imcrop_randcoord, imcrop_randpx, img_pad, img_resize, threshImg)
 from .imgen import (MakeAtom, create_atom_mask_pair, create_lattice_mask,
                     create_multiclass_lattice_mask, create_multiclass_lattice_mask_)
 from .nn import (average_weights, get_downsample_factor, get_nb_classes, gpu_usage_map,

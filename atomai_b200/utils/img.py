@@ -3,7 +3,8 @@ Image helpers on the prediction path (host-side numpy): padding to the network's
 factor, binary thresholding and resizing — atomai/utils/img.py:20-40, 112-135, 554-564; sub-image
 extraction around atoms, and the random patches and patch / spectrum pairs that make training
 sets (atomai/utils/img.py:138-452), whose crops are gathers on the GPU; the blob-size filter of
-segmented frames (atomai/utils/img.py:567-625), labelled on the GPU.
+segmented frames (atomai/utils/img.py:567-625), labelled on the GPU; the FFT-subtraction defect
+map (atomai/utils/img.py:455-499), whose 2-D transforms run on the GPU in float64.
 """
 from numbers import Integral, Real
 from typing import List, Tuple, Union
@@ -117,6 +118,144 @@ def filter_cells(imgdata: np.ndarray,
     each GPU kernel."""
     above = _blob_check(imgdata, 3, im_thresh, blob_thresh, filter_)
     return _filter_blobs(imgdata, im_thresh, blob_thresh, above, imgdata.dtype)
+
+
+# ------------------------------------------------------------------ FFT subtraction
+# atomai/utils/img.py:455-499 runs scipy.fftpack.fft2 / ifft2 on the host.  Here the transforms,
+# the shifts, the disk mask and the normalisation run in csrc/fft.cu, always in float64; a
+# complex64 or float32 result is rounded once, at the store.  The host only checks the arguments
+# and works out the mask's box from the reference's numpy slices.
+_FFT_NP = tuple(np.dtype(t) for t in (
+    np.bool_, np.uint8, np.int8, np.int16, np.uint16, np.int32, np.uint32, np.int64, np.uint64,
+    np.float16, np.float32, np.float64, np.complex64, np.complex128))
+_FFT_SINGLE = tuple(np.dtype(t) for t in (np.float16, np.float32, np.complex64))
+
+
+def _fft_dtype(a) -> np.dtype:
+    """the numpy dtype of a numpy array or CUDA tensor the FFT kernels load; TypeError otherwise"""
+    import torch
+    if _is_cuda(a):
+        from .. import ops
+        if a.dtype not in ops.FFT_CODES:
+            raise TypeError(f"dtype {a.dtype} is not supported by the GPU FFT")
+        return np.dtype(str(a.dtype).replace("torch.", "").replace("bool", "bool_"))
+    if isinstance(a, torch.Tensor) or not isinstance(a, np.ndarray):
+        raise TypeError(f"expected a numpy array or a CUDA tensor, not {type(a)}")
+    if a.dtype not in _FFT_NP:
+        raise TypeError(f"dtype {a.dtype} is not supported by the GPU FFT: it takes bool, integers "
+                        "of up to 64 bits, float16/32/64 and complex64/128")
+    return a.dtype
+
+
+def _fft_shape(shape) -> Tuple[int, int]:
+    """(h, w) of a 2-D image within the transform's size limits; ValueError otherwise"""
+    from .. import _C
+    if len(shape) != 2:
+        raise ValueError(f"the image must be 2-D, got shape {tuple(shape)}")
+    for n in shape:
+        if n < 1:
+            raise ValueError(f"invalid number of data points ({list(shape)}) specified")
+        if n > _C.FFT_MAX_SIDE and (n & (n - 1) or n > _C.FFT_MAX_POW2):
+            raise ValueError(f"a side of {n} is too long for the GPU FFT: at most "
+                             f"{_C.FFT_MAX_SIDE}, or a power of two up to {_C.FFT_MAX_POW2}")
+    return int(shape[0]), int(shape[1])
+
+
+def _mask_box(shape, maskratio) -> Tuple[int, int, int]:
+    """(r0, c0, l) of the disk atomai/utils/img.py:467-471 zeroes: F3[m-l:m+l, m-l:m+l] times
+    (1 - mask) of the (2l, 2l) disk, both from shape[0].  The same expressions raise the same
+    errors (ZeroDivisionError for maskratio=0); slices that do not broadcast with the mask raise
+    ValueError, as numpy does; l = 0 when nothing is masked."""
+    l = int(shape[0] / maskratio)
+    m = int(shape[0] / 2)
+    rows, cols = range(shape[0])[m - l:m + l], range(shape[1])[m - l:m + l]
+    box, mask = (len(rows), len(cols)), (max(2 * l, 0),) * 2
+    try:
+        ok = np.broadcast_shapes(np.broadcast_shapes(box, mask), box) == box
+    except ValueError:
+        ok = False
+    if not ok:
+        raise ValueError(f"the mask of shape {mask} does not broadcast into the slice of shape "
+                         f"{box} (image {tuple(shape)}, maskratio {maskratio})")
+    return (rows.start, cols.start, l) if l > 0 and box == mask else (0, 0, 0)
+
+
+def _to_device(a):
+    import torch
+    if _is_cuda(a):
+        return a.contiguous()
+    if not torch.cuda.is_available():
+        raise RuntimeError("this function runs on a CUDA device; none is available")
+    return torch.from_numpy(np.ascontiguousarray(a)).to("cuda")
+
+
+def _torch_dtype(dt: np.dtype):
+    import torch
+    return torch.from_numpy(np.zeros(0, dt)).dtype
+
+
+def FFTmask(imgsrc: np.ndarray, maskratio: int = 10) -> Tuple[np.ndarray]:
+    """Returns F2, the centred 2-D FFT of an (h, w) image, and F3, a copy of F2 with a disk of
+    radius shape[0] / maskratio zeroed around the centre (atomai/utils/img.py:455-472).  The
+    transform runs on the GPU in float64; F2 and F3 are complex64 for float16, float32 and
+    complex64 input and complex128 otherwise, numpy arrays for numpy input and CUDA tensors for
+    CUDA input.  Each side may be up to 4096 long, or a power of two up to 8192."""
+    import torch
+    from .. import ops
+    from .graphx import _check_free
+    dt = _fft_dtype(imgsrc)
+    h, w = _fft_shape(imgsrc.shape)
+    r0, c0, l = _mask_box(imgsrc.shape, maskratio)
+    out_dt = np.dtype(np.complex64 if dt in _FFT_SINGLE else np.complex128)
+    _check_free(h * w * (2 * out_dt.itemsize + (0 if _is_cuda(imgsrc) else dt.itemsize))
+                + ops.fft2_workspace_bytes(h, w), "FFTmask")
+    img = _to_device(imgsrc)
+    f2 = torch.empty((h, w), dtype=_torch_dtype(out_dt), device=img.device)
+    f3 = torch.empty_like(f2)
+    ops.fft2_mask(img, r0, c0, l, f2, f3)
+    if _is_cuda(imgsrc):
+        return f2, f3
+    return f2.cpu().numpy(), f3.cpu().numpy()
+
+
+def FFTsub(imgsrc: np.ndarray, imgfft: np.ndarray) -> np.ndarray:
+    """Reconstructs an image from the filtered, centred spectrum `imgfft` (complex64 or
+    complex128), subtracts it from `imgsrc` and min-max normalises the absolute difference
+    (atomai/utils/img.py:475-486); a constant difference gives NaN, like the reference's 0 / 0.
+    Both must be 2-D of the same shape.  The result's dtype is the reference's, the real dtype of
+    np.result_type(imgsrc, the spectrum's real dtype), computed in float64 on the GPU; it is a
+    numpy array or a CUDA tensor like `imgsrc`."""
+    import torch
+    from .. import ops
+    from .graphx import _check_free
+    src_dt, fft_dt = _fft_dtype(imgsrc), _fft_dtype(imgfft)
+    if fft_dt.kind != "c":
+        raise TypeError(f"imgfft must be a complex64 or complex128 spectrum, not {fft_dt}")
+    h, w = _fft_shape(imgsrc.shape)
+    if tuple(imgfft.shape) != (h, w):
+        raise ValueError(f"imgsrc {tuple(imgsrc.shape)} and imgfft {tuple(imgfft.shape)} must "
+                         "have the same 2-D shape")
+    out_dt = np.result_type(src_dt, np.empty(0, fft_dt).real.dtype)
+    out_dt = np.empty(0, out_dt).real.dtype
+    _check_free(h * w * (out_dt.itemsize + (0 if _is_cuda(imgsrc) else src_dt.itemsize)
+                         + (0 if _is_cuda(imgfft) else fft_dt.itemsize))
+                + ops.fft2_workspace_bytes(h, w), "FFTsub")
+    src = _to_device(imgsrc)
+    spec = _to_device(imgfft).to(src.device)
+    out = torch.empty((h, w), dtype=_torch_dtype(out_dt), device=src.device)
+    ops.fft2_sub(src, spec, out)
+    return out if _is_cuda(imgsrc) else out.cpu().numpy()
+
+
+def threshImg(diff: np.ndarray,
+              threshL: float = 0.25,
+              threshH: float = 0.75) -> np.ndarray:
+    """Marks the pixels of `diff` below threshL or above threshH as defects
+    (atomai/utils/img.py:489-499): a bool array, or a bool tensor for a tensor input."""
+    import torch
+    if isinstance(diff, torch.Tensor):
+        return torch.logical_or(diff < threshL, diff > threshH)
+    return (diff < threshL) + (diff > threshH)
 
 
 def img_resize(image_data: np.ndarray, rs: Tuple[int], round_: bool = False) -> np.ndarray:

@@ -465,6 +465,40 @@ int atomai_b200_imgen_fill(const int32_t* atoms, const int64_t* frames, int F, i
 int atomai_b200_blob_filter(const void* img, int dtype, int64_t n, int h, int w, double im_thresh,
                             double blob_thresh, int above, int32_t* labels, int32_t* counts,
                             void* out, int out_dtype, void* stream);
+/* ---- 2-D FFTs of utils.FFTmask / FFTsub (atomai/utils/img.py:455-486) ------------------------
+ * float64 complex transforms of one row-major (h, w) array; each side is in [1, AB_FFT_MAX_SIDE]
+ * or a power of two up to AB_FFT_MAX_POW2.  Lengths that are not powers of two run by Bluestein's
+ * chirp-z method.  `work` is caller-owned device scratch of at least
+ * atomai_b200_fft2_workspace_bytes(h, w) bytes (-1 for an unsupported side), 256 B aligned.
+ * Element dtypes: AB_FFT_U8 .. AB_FFT_C128 (bool as AB_FFT_U8).  All passes run on `stream`.
+ * fft2_mask: F2 = fftshift(fft2(img)); F3 = F2 except F3 = F2 * (1 - disk) at (r0 + y, c0 + x),
+ *   0 <= x, y < 2l, disk = (x + 1 - l)^2 + (y + 1 - l)^2 <= l^2 (l = 0: F3 = F2).  f2 and f3 are
+ *   (h, w) complex64 (c64 != 0, each component rounded once) or complex128.
+ * fft2_sub: recon = Re(ifft2(ifftshift(spec))) with the 1 / (h w) scale, spec complex64 or
+ *   complex128; d = |img - recon|; out = (d - min d) / (max d - min d) in float64 (NaN-propagating
+ *   extremes, a constant d gives NaN), stored as float32 (out_f32 != 0) or float64. */
+#define AB_FFT_U8 0
+#define AB_FFT_I8 1
+#define AB_FFT_I16 2
+#define AB_FFT_U16 3
+#define AB_FFT_I32 4
+#define AB_FFT_U32 5
+#define AB_FFT_I64 6
+#define AB_FFT_U64 7
+#define AB_FFT_F16 8
+#define AB_FFT_F32 9
+#define AB_FFT_F64 10
+#define AB_FFT_C64 11
+#define AB_FFT_C128 12
+#define AB_FFT_MAX_SIDE 4096
+#define AB_FFT_MAX_POW2 8192
+int64_t atomai_b200_fft2_workspace_bytes(int h, int w);
+int atomai_b200_fft2_mask(const void* img, int dtype, int h, int w, int r0, int c0, int l,
+                          void* f2, void* f3, int c64, void* work, int64_t work_bytes,
+                          void* stream);
+int atomai_b200_fft2_sub(const void* img, int img_dtype, const void* spec, int spec_dtype, int h,
+                         int w, void* out, int out_f32, void* work, int64_t work_bytes,
+                         void* stream);
 /* 2-D Gaussian peak refinement (atomai/utils/coords.py:152-231, predictors/predictor.py:609-619):
  * for each of the K rows {frame, row0, col0, d} of `atoms` (int32, device) one least-squares fit of
  *   offset + amp exp(-(a (x-xo)^2 + 2 b (x-xo)(y-yo) + c (y-yo)^2))
