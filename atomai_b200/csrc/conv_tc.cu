@@ -92,6 +92,12 @@ struct ConvTcParams {
   int tma;
   int raw_bytes;     // HP * KC * 4
   int n_r;           // raw stages (two rings of n_r/2)
+  // tiles per consumer pass (1 or 2).  2: a consumer takes two of its tiles at once, k-chunk by
+  // k-chunk, and issues every (tap, k-step) MMA of one tile right after the same MMA of the
+  // other, so two independent accumulator chains hide each other's wgmma latency.  Every tile
+  // keeps its own accumulators, MMA order and place in the statistics token sequence, so outputs
+  // and statistics are bit-identical to pair = 1.
+  int pair;
 };
 
 struct __align__(8) SharedCtl {
@@ -130,7 +136,9 @@ __device__ __forceinline__ void bulk_g2s_if(uint32_t pred, uint32_t dst_smem, co
 // core always has the next group queued.  A streamed weight stage is refilled at that point by
 // the consumer's first thread with the piece it holds next (n_b/2 pieces ahead): the retired group
 // was issued by all four warps, so none of them still waits for the stage's previous contents.
-template <int N, int SUB, int PIPE>
+// PAIR = 2 (resident weights, see ConvTcParams::pair) runs its own pass loop below; the PAIR = 1
+// tile loop is not touched by it.
+template <int N, int SUB, int PAIR, int PIPE>
 __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* ctl, uint32_t a_base,
                                               uint32_t b_base, float* s_stats, const float* s_bias) {
   // PIPE is a template parameter: control flow that depends on the thread index puts the MMAs on
@@ -355,7 +363,166 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
     }
   };
 
-  for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += tile_step) tile_fn(tile);
+  if constexpr (PAIR == 1) {
+    for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += tile_step) tile_fn(tile);
+  } else {
+    // A pass takes the consumer's tiles k and k + 1 (tile, tile + tile_step); the loaders stage
+    // them k-chunk by k-chunk, one operand stage each, so a pass holds both stages of its
+    // pipeline and every k-chunk group retires right after its commit (the other pipeline keeps
+    // the tensor core busy meanwhile; a wgmma wait at the top of the chunk instead makes ptxas
+    // serialise the MMAs).  A lone last tile is staged twice and the second result dropped, so
+    // no MMA or wgmma wait depends on whether the pass has two tiles.  Both tiles' epilogues run
+    // before the first statistics add: accumulators read after the lane-dependent adds also
+    // serialise the MMAs.
+    constexpr int JL = (R / 4 + 7) / 8;
+    const int c_lane = 2 * (lane & 3);
+    float pacc[2][SUB][MB][R];
+    // tile `tl`'s epilogue from accumulators `a`, as tile_fn's; `real` = 0: the dropped second
+    // tile, which stores nothing.  Its channel sums go to `st` for add_stats.
+    auto pair_epilogue = [&](float (&a)[SUB][MB][R], const int tl, const bool real, float (&st)[JL][4]) {
+      const int n = tl / tpi, rem = tl - n * tpi;
+      const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
+      auto epilogue = [&](auto fast_tag) {
+        constexpr bool FAST = decltype(fast_tag)::value;
+#pragma unroll
+        for (int j = 0; j < R / 4; ++j) {
+          const int c = p.n0 + 8 * j + c_lane;
+          const float b0 = s_bias[c], b1 = s_bias[c + 1];
+          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+          for (int s = 0; s < SUB; ++s)
+#pragma unroll
+            for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+              for (int hrow = 0; hrow < 2; ++hrow) {
+                const int gh = th_i * kTileH + mb * 8 + 2 * warp + hrow;
+                const int gw = (tw_i * SUB + s) * kTileW + (lane >> 2);
+                const bool valid = real && gh < p.H && gw < p.W;
+                float v0 = a[s][mb][4 * j + 2 * hrow] + b0, v1 = a[s][mb][4 * j + 2 * hrow + 1] + b1;
+                if (FAST) {
+                  v0 = fmaxf(v0, v0 * alpha);
+                  v1 = fmaxf(v1, v1 * alpha);
+                } else if (p.act == AB_ACT_RBF) {
+                  v0 = alpha * exp2f(-0.72134752f * fmaxf(v0, 0.f));
+                  v1 = alpha * exp2f(-0.72134752f * fmaxf(v1, 0.f));
+                } else {
+                  v0 = act_f(v0, p.act, alpha);
+                  v1 = act_f(v1, p.act, alpha);
+                }
+                v0 = valid ? v0 : 0.f;
+                v1 = valid ? v1 : 0.f;
+                if (valid) {
+                  const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
+                  if (!p.out_nchw) {
+                    *reinterpret_cast<float2*>(p.out + pix * p.ld_out + c) = make_float2(v0, v1);
+                  } else {
+                    const size_t hw = (size_t)p.nchw_stride;
+                    float* o = p.out + ((size_t)n * p.Cout + c) * hw + (size_t)gh * p.W + gw;
+                    o[0] = v0;
+                    o[hw] = v1;
+                  }
+                }
+                s0 += v0; s1 += v1;
+                q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
+              }
+          if (p.stats) {
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+              s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+              s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+              q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+              q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+            }
+            if ((lane >> 2) == (j & 7)) {
+              st[j >> 3][0] = s0; st[j >> 3][1] = s1; st[j >> 3][2] = q0; st[j >> 3][3] = q1;
+            }
+          }
+        }
+      };
+      if (fast) epilogue(std::true_type{});
+      else epilogue(std::false_type{});
+    };
+    // tile `tl`'s statistics, added in tile order as tile_fn does
+    auto add_stats = [&](const int tl, const float (&st)[JL][4]) {
+      if (tl != (int)blockIdx.x) named_bar_sync(kStatBar + (PIPE ? 0 : kNumEpiWarps) + warp, 64);
+#pragma unroll
+      for (int jl = 0; jl < JL; ++jl) {
+        const int j = 8 * jl + (lane >> 2);
+        if (j < R / 4) {
+          const int c = p.n0 + 8 * j + c_lane;
+          my_stats[c] += st[jl][0];
+          my_stats[c + 1] += st[jl][1];
+          my_stats[p.Cout + c] += st[jl][2];
+          my_stats[p.Cout + c + 1] += st[jl][3];
+        }
+      }
+      if (tl + (int)gridDim.x < p.num_tiles)
+        named_bar_arrive(kStatBar + (PIPE ? kNumEpiWarps : 0) + warp, 64);
+    };
+    auto pass_fn = [&](const int tile) {
+      const bool two = tile + tile_step < p.num_tiles;
+      uint32_t accum = 0;
+      for (int ch = 0; ch < p.n_chunks; ++ch) {
+        uint32_t a_stage[2], empty[2];
+#pragma unroll
+        for (int w = 0; w < 2; ++w) {
+          mbar_wait_quiet(bar_full_a + (ring0 + s_a) * 8, p_a);
+          a_stage[w] = a_base + (ring0 + s_a) * p.a_stage_bytes;
+          empty[w] = bar_empty_a + (ring0 + s_a) * 8;
+          if (++s_a == ring_n) { s_a = 0; p_a ^= 1; }
+        }
+        for (int t = 0; t < taps; ++t) {
+          const int ty = t / tw, tx = t - ty * tw;
+          const uint32_t tap_off = (uint32_t)(ty * p.TWp + tx) * p.dil * 16;
+          wgmma_fence();
+          for (int ks = 0; ks < ksteps; ++ks) {
+            const uint32_t a_k = tap_off + ks * 2u * p.plane_bytes;
+            const uint32_t b_k = b_n0 + b_base + ((uint32_t)(ch * ksteps + ks) * wmult * taps + t) * piece;
+            const uint64_t bd = b_tmpl | (b_k >> 4);
+#pragma unroll
+            for (int w = 0; w < 2; ++w)
+#pragma unroll
+              for (int s = 0; s < SUB; ++s)
+#pragma unroll
+                for (int mb = 0; mb < MB; ++mb)
+                  Wgmma<N>::tf32(pacc[w][s][mb],
+                                 a_tmpl | ((a_stage[w] + a_k + mb * mb_off + s * sb_off) >> 4), bd, accum);
+            if (x3) {
+              const uint64_t bc = b_tmpl | ((b_k + corr_w) >> 4);
+#pragma unroll
+              for (int w = 0; w < 2; ++w)
+#pragma unroll
+                for (int s = 0; s < SUB; ++s)
+#pragma unroll
+                  for (int mb = 0; mb < MB; ++mb)
+                    Wgmma<N>::bf16(pacc[w][s][mb],
+                                   a_tmpl | ((a_stage[w] + a_k + p.corr_off + mb * mb_off + s * sb_off) >> 4),
+                                   bc, 1u);
+            }
+            accum = 1u;
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        consumer_release(empty[0]);
+        consumer_release(empty[1]);
+      }
+#pragma unroll
+      for (int w = 0; w < 2; ++w)
+#pragma unroll
+        for (int s = 0; s < SUB; ++s)
+#pragma unroll
+          for (int mb = 0; mb < MB; ++mb) wgmma_fence_regs(pacc[w][s][mb]);
+      float st[2][JL][4];
+#pragma unroll
+      for (int w = 0; w < 2; ++w) pair_epilogue(pacc[w], tile + w * tile_step, w == 0 || two, st[w]);
+      if (p.stats) {
+        add_stats(tile, st[0]);
+        if (two) add_stats(tile + tile_step, st[1]);
+      }
+    };
+    for (int tile = blockIdx.x + pipe * gridDim.x; tile < p.num_tiles; tile += 2 * tile_step) pass_fn(tile);
+  }
   if (p.stats) {   // this CTA's partial = the four warps' sums in warp order, then ordered over CTAs
     constexpr int kNt = kNumConsWarps * 32;
     auto bar = [] { asm volatile("bar.sync 1, %0;" ::"n"(kNt) : "memory"); };
@@ -401,7 +568,7 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm,
       : "memory");
 }
 
-template <int U>
+template <int U, int PAIR>
 __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ctl,
                                             uint32_t a_base, uint32_t raw_base, int grp,
                                             const CUtensorMap* tm0, const CUtensorMap* tm1) {
@@ -439,7 +606,13 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
   const uint32_t ring_n = dual ? n_a / 2 : n_a;
   const uint32_t ring0 = dual ? grp * ring_n : 0u;
   int tile = dual ? blockIdx.x + grp * gridDim.x : blockIdx.x;
-  const int n_chunks_eff = n_chunks;
+  // PAIR = 2: a pass covers the group's tiles `tile` and tile + tile_step, k-chunk by k-chunk in
+  // the order its consumer takes them: pass chunk ch is k-chunk ch / 2 of the pass's tile ch % 2
+  // (`tile` again when tile + tile_step is past the end)
+  const int n_chunks_eff = n_chunks * PAIR;
+  auto tile_of = [&](int r_tile, int r_ch) {
+    return PAIR == 2 && (r_ch & 1) && r_tile + tile_step < p.num_tiles ? r_tile + tile_step : r_tile;
+  };
   // x3: besides the TF32 planes every element also goes, as bf16, into the correction planes of
   // its k-step: plane 2*ks holds the low parts a - rn_tf32(a) of the 8 channels, plane 2*ks + 1
   // the high parts (one 16-byte row per pixel each = one K-major core-matrix row of a K = 16 MMA).
@@ -468,26 +641,27 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
   // the group's k-chunk `ahead` chunks after (r_tile, r_ch), or r_tile >= num_tiles past its last
   auto chunk_after = [&](int& r_tile, int& r_ch, int ahead) {
     r_ch += ahead;
-    while (r_ch >= n_chunks) { r_ch -= n_chunks; r_tile += tile_step; }
+    while (r_ch >= n_chunks_eff) { r_ch -= n_chunks_eff; r_tile += PAIR * tile_step; }
   };
   if (p.tma && gt == 0) {   // the first rn chunks; after that, one per transformed chunk
     for (uint32_t i = 0; i < rn; ++i) {
       int r_tile = tile, r_ch = 0;
       chunk_after(r_tile, r_ch, (int)i);
-      if (r_tile < p.num_tiles) issue_raw(r_tile, r_ch, i);
+      if (r_tile < p.num_tiles) issue_raw(tile_of(r_tile, r_ch), r_ch / PAIR, i);
     }
   }
   int ch = dual ? 0 : grp;
   uint32_t st = dual ? 0u : grp % n_a;
   uint32_t ph = dual ? 1u : ((grp / n_a) & 1) ^ 1;   // stage / empty-phase of the current chunk
   for (;;) {
-    while (ch >= n_chunks_eff) { ch -= n_chunks_eff; tile += tile_step; }
+    while (ch >= n_chunks_eff) { ch -= n_chunks_eff; tile += PAIR * tile_step; }
     if (tile >= p.num_tiles) break;
-    const int ch_real = ch;
-    // tile -> (n, th_i, tw_i) without integer division
-    int n = __float2int_rz((float)tile * inv_tpi);
-    n += ((n + 1) * tpi <= tile) - (n * tpi > tile);
-    const int rem = tile - n * tpi;
+    const int ch_real = ch / PAIR;
+    const int cur = tile_of(tile, ch);   // the tile this chunk belongs to
+    // cur -> (n, th_i, tw_i) without integer division
+    int n = __float2int_rz((float)cur * inv_tpi);
+    n += ((n + 1) * tpi <= cur) - (n * tpi > cur);
+    const int rem = cur - n * tpi;
     int th_i = __float2int_rz((float)rem * inv_tw);
     th_i += ((th_i + 1) * p.tiles_w <= rem) - (th_i * p.tiles_w > rem);
     const int tw_i = rem - th_i * p.tiles_w;
@@ -653,7 +827,7 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
         chunk_after(r_tile, r_ch, (int)rn);
         if (r_tile < p.num_tiles) {
           mbar_wait_quiet(bar_raw_empty + (rr0 + rst) * 8, rph);
-          issue_raw(r_tile, r_ch, rst);
+          issue_raw(tile_of(r_tile, r_ch), r_ch / PAIR, rst);
         }
       }
       if (++rst == rn) { rst = 0; rph ^= 1; }
@@ -669,17 +843,22 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
 template <int PIPE>
 __device__ __forceinline__ void conv_consumer(const ConvTcParams& p, SharedCtl* ctl, uint32_t a_base,
                                               uint32_t b_base, float* s_stats, const float* s_bias) {
-#define AB_CONS_CASE(NN, S) \
-  case NN: consumer_loop<NN, S, PIPE>(p, ctl, a_base, b_base, s_stats, s_bias); break;
-  if (p.sub == 2) {
+#define AB_CONS_CASE(NN, S, T) \
+  case NN: consumer_loop<NN, S, T, PIPE>(p, ctl, a_base, b_base, s_stats, s_bias); break;
+  if (p.pair == 2) {
     switch (p.nn) {
-      AB_CONS_CASE(16, 2) AB_CONS_CASE(32, 2) AB_CONS_CASE(48, 2) AB_CONS_CASE(64, 2)
+      AB_CONS_CASE(16, 1, 2) AB_CONS_CASE(32, 1, 2)
+      default: __trap();
+    }
+  } else if (p.sub == 2) {
+    switch (p.nn) {
+      AB_CONS_CASE(16, 2, 1) AB_CONS_CASE(32, 2, 1) AB_CONS_CASE(48, 2, 1) AB_CONS_CASE(64, 2, 1)
       default: __trap();
     }
   } else {
     switch (p.nn) {
-      AB_CONS_CASE(16, 1) AB_CONS_CASE(32, 1) AB_CONS_CASE(48, 1) AB_CONS_CASE(64, 1)
-      AB_CONS_CASE(80, 1) AB_CONS_CASE(96, 1) AB_CONS_CASE(112, 1) AB_CONS_CASE(128, 1)
+      AB_CONS_CASE(16, 1, 1) AB_CONS_CASE(32, 1, 1) AB_CONS_CASE(48, 1, 1) AB_CONS_CASE(64, 1, 1)
+      AB_CONS_CASE(80, 1, 1) AB_CONS_CASE(96, 1, 1) AB_CONS_CASE(112, 1, 1) AB_CONS_CASE(128, 1, 1)
       default: __trap();
     }
   }
@@ -734,8 +913,14 @@ __global__ void __launch_bounds__(kThreads, 1)
     // compiler keeps all of them in flight before the first use.
     const int grp = (warp - kFirstLoadWarp) >> 2;
     const int U = (p.HP * (p.KC >> 2) + kGroupThreads - 1) / kGroupThreads;   // <= kMaxU (plan)
-    switch (U) {
-#define AB_LOAD_CASE(K) case K: loader_loop<K>(p, ctl, a_base, raw_base, grp, &tm0, &tm1); break;
+    if (p.pair == 2) {   // the plan pairs only these element counts
+      switch (U) {
+        case 2: loader_loop<2, 2>(p, ctl, a_base, raw_base, grp, &tm0, &tm1); break;
+        case 4: loader_loop<4, 2>(p, ctl, a_base, raw_base, grp, &tm0, &tm1); break;
+        default: __trap();
+      }
+    } else switch (U) {
+#define AB_LOAD_CASE(K) case K: loader_loop<K, 1>(p, ctl, a_base, raw_base, grp, &tm0, &tm1); break;
       AB_LOAD_CASE(1) AB_LOAD_CASE(2) AB_LOAD_CASE(3) AB_LOAD_CASE(4) AB_LOAD_CASE(5) AB_LOAD_CASE(6)
       AB_LOAD_CASE(7) AB_LOAD_CASE(8) AB_LOAD_CASE(9) AB_LOAD_CASE(10) AB_LOAD_CASE(11)
       AB_LOAD_CASE(12)
@@ -854,6 +1039,7 @@ struct PlanKnobs {
   bool tma = true;           // ATOMAI_B200_TMA=0: register-staged loaders only
   int res_na4 = -1;          // ATOMAI_B200_RES_NA4=0/1: resident n_a = 4 rule for no / every layer
   int tma_min_kc = 16;       // ATOMAI_B200_TMA_KC8 (set): TMA plans may use 32-byte box rows
+  bool pair = true;          // ATOMAI_B200_PAIR=0: thin layers take one tile per consumer pass
   bool log = false;          // ATOMAI_B200_PLAN_LOG (set): print every plan to stderr
 };
 
@@ -869,6 +1055,7 @@ static PlanKnobs plan_knobs() {
   if (const char* e = getenv("ATOMAI_B200_TMA")) k.tma = e[0] != '0';
   if (const char* e = getenv("ATOMAI_B200_RES_NA4")) k.res_na4 = e[0] == '1' ? 1 : 0;
   if (getenv("ATOMAI_B200_TMA_KC8")) k.tma_min_kc = 8;
+  if (const char* e = getenv("ATOMAI_B200_PAIR")) k.pair = e[0] != '0';
   k.log = getenv("ATOMAI_B200_PLAN_LOG") != nullptr;
   return k;
 }
@@ -1010,6 +1197,19 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
   AB_CHECK(ok, "conv_tc: no shared-memory plan (Cin=%d Cout=%d dil=%d)", S.Ctot, d->Cout, d->dil);
   p->num_tiles = d->N * p->tiles_h * p->tiles_w;
   p->n_chunks = S.Ctot / p->KC;
+  // Thin 3x3 layers (one launch of <= 32 channels: at most 32 accumulator registers per tile)
+  // issue the MMAs of two tiles back to back.  A pass holds one operand stage per tile, so the
+  // pipeline's ring must have two; a pipeline needs two tiles for a pass to add a chain (with
+  // num_tiles <= 2 * grid every pass would be a lone tile, staged and multiplied twice); the
+  // loader has paired instantiations for 2 and 4 elements per thread only (KC = 8 / 16 at
+  // dilation 1).  A 1x1 layer's k-chunk is too few MMAs to pay for retiring every group before
+  // the next chunk is staged.
+  {
+    const int u = (p->HP * (p->KC >> 2) + kGroupThreads - 1) / kGroupThreads;
+    const int sms = ab_num_sms(), grid = p->num_tiles < sms ? p->num_tiles : sms;
+    p->pair = (k.pair && p->w_resident && p->sub == 1 && d->Cout <= 32 && p->n_a == 4 && taps > 1 &&
+               p->num_tiles > 2 * grid && (u == 2 || u == 4)) ? 2 : 1;
+  }
   AB_CHECK(p->plane_bytes / 16 < (1 << 14) && p->TWp < (1 << 14), "conv_tc: descriptor overflow");
   *smem_bytes = plan_smem(*p, stats_bytes);
   if (k.log)
@@ -1018,6 +1218,8 @@ static int conv_tc_plan(const ab_conv_t* d, ConvTcParams* p, int* smem_bytes) {
             "n_b=%d tma=%d n_r=%d a_stage=%d smem=%d\n",
             d->H, d->W, S.Ctot, d->Cout, taps, p->x3, p->w_resident, p->sub, p->KC, p->n_a, p->n_b,
             p->tma, p->n_r, p->a_stage_bytes, *smem_bytes);
+  if (k.log)
+    fprintf(stderr, "conv_tc tile: 8x%d px, %d tile(s) per consumer pass\n", kTileW * p->sub, p->pair);
   return 0;
 }
 
