@@ -58,6 +58,30 @@ __device__ __forceinline__ void cta_slots_finish(const Ordered& red, int group, 
                  s_last);
 }
 
+// The same for a 256-thread quad-lane kernel (lane = pixel l >> 2 of an 8-pixel run x quad l & 3)
+// with one slot of 4 * NV partials per warp: each of the thread's NV values val(i) is summed over
+// the warp's 8 pixel lanes, lane q < 4 stores the total at slot(q, i), and the last CTA adds the
+// slots in (CTA, warp) order and hands each total to add(i, sum).
+template <int NV, class Val, class Slot, class Add>
+__device__ __forceinline__ void quad_slots_finish(const Ordered& red, Val val, Slot slot, Add add,
+                                                  unsigned* s_last) {
+  const int lane = threadIdx.x & 31;
+  double* dst = ordered_slot(red, 0, gridDim.x * 8, blockIdx.x * 8 + (threadIdx.x >> 5), 4 * NV);
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    float v = val(i);
+#pragma unroll
+    for (int m = 4; m <= 16; m <<= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
+    if (lane < 4) dst[slot(lane, i)] = v;
+  }
+  ordered_finish(red, 0, gridDim.x * 8, 4 * NV, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
+                 add, s_last);
+}
+// slot layout [i / 4][quad][i % 4] of 4 x 4 values per quad (the BN sums then the squares of a
+// quad's 4 channels; dW[output][input quad][4 inputs])
+__device__ __forceinline__ int quad_stat_slot(int q, int i) { return (i >> 2) * 16 + q * 4 + (i & 3); }
+
 __global__ void __launch_bounds__(F_THREADS) conv_simt_fwd_kernel(const ConvSimtParams p) {
   extern __shared__ float sm[];
   const int taps = p.th * p.tw;
@@ -535,35 +559,17 @@ __global__ void __launch_bounds__(256) conv_c1_tile_kernel(const ConvSimtParams 
       }
     }
   }
-  if (p.stats) {
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      float a = ssum[k], b = ssq[k];
-#pragma unroll
-      for (int m = 4; m <= 16; m <<= 1) {
-        a += __shfl_xor_sync(0xffffffffu, a, m);
-        b += __shfl_xor_sync(0xffffffffu, b, m);
-      }
-      if (lane < 4) {   // one slot per warp, added in (CTA, warp) order
-        double* slot = ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + (threadIdx.x >> 5), 32);
-        slot[q * 4 + k] = a;
-        slot[16 + q * 4 + k] = b;
-      }
-    }
-    ordered_finish(p.red, 0, gridDim.x * 8, 32, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
-                   [&](int i, double v) { p.stats[(i < 16 ? c0 : p.Cout + c0 - 16) + i] += v; },
-                   &s_last);
-  }
+  if (p.stats)
+    quad_slots_finish<8>(p.red, [&](int i) { return i < 4 ? ssum[i] : ssq[i - 4]; }, quad_stat_slot,
+                         [&](int i, double v) { p.stats[(i < 16 ? c0 : p.Cout + c0 - 16) + i] += v; },
+                         &s_last);
 }
 
 int launch_conv_c1_tile(const ConvSimtParams& p, cudaStream_t stream) {
   const int tiles_w = (p.W + C1T_W - 1) / C1T_W, tiles_h = (p.H + C1T_H - 1) / C1T_H;
   const int64_t tiles = (int64_t)p.N * tiles_w * tiles_h;
   AB_CHECK(tiles < (1ll << 31), "conv_c1: too many tiles");
-  int64_t blocks = tiles;
-  const int64_t cap = (int64_t)ab_num_sms() * 3;
-  if (blocks > cap) blocks = cap;
+  const int64_t blocks = ab_grid(tiles, 1, 3);
   const bool fast = p.act == AB_ACT_LRELU && p.alpha >= 0.f && p.alpha <= 1.f;
   ConvSimtParams q = p;
   if (p.stats && ab_ordered_ws(stream, blocks * 8 * 32, 1, &q.red)) return 1;
@@ -579,10 +585,7 @@ template <int CO>
 int launch_conv_c1(const ConvSimtParams& p, cudaStream_t stream) {
   const int64_t pairs = (int64_t)p.N * p.H * ((p.W + 1) / 2);
   AB_CHECK(pairs < (1ll << 31), "conv_c1: too many pixels");
-  int64_t blocks = (pairs + 255) / 256;
-  const int64_t cap = (int64_t)ab_num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const int64_t blocks = ab_grid(pairs, 256, 16);
   ConvSimtParams q = p;
   if (p.stats && ab_ordered_ws(stream, blocks * 2 * CO, 1, &q.red)) return 1;
   conv_c1_kernel<CO><<<(unsigned)blocks, 256, 0, stream>>>(q);
@@ -650,33 +653,14 @@ __global__ void __launch_bounds__(256) conv_pix_quad_kernel(const ConvSimtParams
     *reinterpret_cast<float4*>(p.out + pix * p.ld_out + q * 4) = make_float4(a[0], a[1], a[2], a[3]);
   }
   (void)px;
-  if (p.stats) {
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      float a = ssum[k], b = ssq[k];
-#pragma unroll
-      for (int m = 4; m <= 16; m <<= 1) {
-        a += __shfl_xor_sync(0xffffffffu, a, m);
-        b += __shfl_xor_sync(0xffffffffu, b, m);
-      }
-      if (lane < 4) {   // one slot per warp, added in (CTA, warp) order
-        double* slot = ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + (threadIdx.x >> 5), 32);
-        slot[q * 4 + k] = a;
-        slot[16 + q * 4 + k] = b;
-      }
-    }
-    ordered_finish(p.red, 0, gridDim.x * 8, 32, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
-                   [&](int i, double v) { p.stats[(i < 16 ? 0 : p.Cout - 16) + i] += v; }, &s_last);
-  }
+  if (p.stats)
+    quad_slots_finish<8>(p.red, [&](int i) { return i < 4 ? ssum[i] : ssq[i - 4]; }, quad_stat_slot,
+                         [&](int i, double v) { p.stats[(i < 16 ? 0 : p.Cout - 16) + i] += v; }, &s_last);
 }
 
 int launch_conv_pix_quad(const ConvSimtParams& p, cudaStream_t stream) {
   const int64_t npix = (int64_t)p.N * p.H * p.W;
-  int64_t blocks = (npix * 4 + 256 * 8 - 1) / (256 * 8);
-  const int64_t cap = (int64_t)ab_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const int64_t blocks = ab_grid(npix * 4, 256 * 8, 8);
   ConvSimtParams q = p;
   if (p.stats && ab_ordered_ws(stream, blocks * 8 * 32, 1, &q.red)) return 1;
   if (p.S.Ctot <= 4) conv_pix_quad_kernel<4><<<(unsigned)blocks, 256, 0, stream>>>(q);
@@ -694,10 +678,7 @@ int launch_conv_pix(const ConvSimtParams& p, cudaStream_t stream) {
   int vec = (Cin % 4 == 0);
   for (int i = 0; i < p.S.nsrc; ++i)
     if (p.S.s[i].C % 4 != 0 || p.S.s[i].ld % 4 != 0 || ((uintptr_t)p.S.s[i].ptr & 15)) vec = 0;
-  int64_t blocks = (npix + 256 * 4 - 1) / (256 * 4);
-  const int64_t cap = (int64_t)ab_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const int64_t blocks = ab_grid(npix, 256 * 4, 8);
   ConvSimtParams q = p;
   if (p.stats && ab_ordered_ws(stream, blocks * 2 * CO, 1, &q.red)) return 1;
   conv_pix_kernel<CO><<<(unsigned)blocks, 256, smem, stream>>>(q, vec);
@@ -919,29 +900,17 @@ __global__ void __launch_bounds__(256) wgrad_c1_tile_kernel(const WgradSimtParam
       }
     }
   }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < 4; ++k)
-#pragma unroll
-    for (int t = 0; t < 9; ++t) {
-      float v = acc[k][t];
-#pragma unroll
-      for (int m = 4; m <= 16; m <<= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
-      if (lane < 4)     // one slot per warp, added in (CTA, warp) order
-        ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + warp, 16 * 9)[(q * 4 + k) * 9 + t] = v;
-    }
   __shared__ unsigned s_last;
-  ordered_finish(p.red, 0, gridDim.x * 8, 16 * 9, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
-                 [&](int i, double v) { p.dw[i] += (float)v; }, &s_last);   // OIHW, Cin = 1
+  quad_slots_finish<4 * 9>(p.red, [&](int i) { return acc[i / 9][i % 9]; },
+                           [](int q, int i) { return q * 4 * 9 + i; },   // dW[channel q*4 + i/9][tap i%9]
+                           [&](int i, double v) { p.dw[i] += (float)v; }, &s_last);   // OIHW, Cin = 1
 }
 
 int launch_wgrad_c1_tile(const WgradSimtParams& p, cudaStream_t stream) {
   const int tiles_w = (p.W + C1T_W - 1) / C1T_W, tiles_h = (p.H + C1T_H - 1) / C1T_H;
   const int64_t tiles = (int64_t)p.N * tiles_w * tiles_h;
   AB_CHECK(tiles < (1ll << 31), "wgrad_c1: too many tiles");
-  int64_t blocks = tiles;
-  const int64_t cap = (int64_t)ab_num_sms() * 3;
-  if (blocks > cap) blocks = cap;
+  const int64_t blocks = ab_grid(tiles, 1, 3);
   WgradSimtParams q = p;
   if (ab_ordered_ws(stream, blocks * 8 * 16 * 9, 1, &q.red)) return 1;
   wgrad_c1_tile_kernel<<<(unsigned)blocks, 256, 0, stream>>>(q, tiles_w, tiles_w * tiles_h, (int)tiles);
@@ -959,10 +928,7 @@ template <int CO>
 int launch_wgrad_c1(const WgradSimtParams& p, cudaStream_t stream) {
   const int64_t pairs = (int64_t)p.N * p.H * ((p.W + 1) / 2);
   AB_CHECK(pairs < (1ll << 31), "wgrad_c1: too many pixels");
-  int64_t bx = (pairs + 256 * 8 - 1) / (256 * 8);
-  const int64_t cap = (int64_t)ab_num_sms() * 4;
-  if (bx > cap) bx = cap;
-  if (bx < 1) bx = 1;
+  const int64_t bx = ab_grid(pairs, 256 * 8, 4);
   dim3 grid((unsigned)bx, 2, 1);
   WgradSimtParams q = p;
   if (ab_ordered_ws(stream, bx * 2 * (CO / 2) * 9, 2, &q.red)) return 1;
@@ -1080,28 +1046,14 @@ __global__ void __launch_bounds__(256) wgrad_pix_quad_kernel(const WgradSimtPara
       for (int b = 0; b < 4; ++b) acc[a][b] = fmaf(d, x[b], acc[a][b]);
     }
   }
-  __syncthreads();
-#pragma unroll
-  for (int a = 0; a < 4; ++a)
-#pragma unroll
-    for (int b = 0; b < 4; ++b) {
-      float v = acc[a][b];
-#pragma unroll
-      for (int m = 4; m <= 16; m <<= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
-      if (lane < 4)     // one slot per warp, added in (CTA, warp) order
-        ordered_slot(p.red, 0, gridDim.x * 8, blockIdx.x * 8 + (threadIdx.x >> 5), 64)[a * 16 + q * 4 + b] = v;
-    }
   __shared__ unsigned s_last;
-  ordered_finish(p.red, 0, gridDim.x * 8, 64, threadIdx.x, 256, gridDim.x, [] { __syncthreads(); },
-                 [&](int i, double v) { if ((i >> 4) < Cout) p.dw[(size_t)(i >> 4) * 16 + (i & 15)] += (float)v; },
-                 &s_last);                                            // OIHW with 1x1 taps
+  quad_slots_finish<16>(p.red, [&](int i) { return acc[i >> 2][i & 3]; }, quad_stat_slot,
+                        [&](int i, double v) { if ((i >> 4) < Cout) p.dw[(size_t)(i >> 4) * 16 + (i & 15)] += (float)v; },
+                        &s_last);                                     // OIHW with 1x1 taps
 }
 
 int launch_wgrad_pix_quad(const WgradSimtParams& p, cudaStream_t stream) {
-  int64_t blocks = (p.npix * 4 + 256 * 8 - 1) / (256 * 8);
-  const int64_t cap = (int64_t)ab_num_sms() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const int64_t blocks = ab_grid(p.npix * 4, 256 * 8, 8);
   WgradSimtParams q = p;
   if (ab_ordered_ws(stream, blocks * 8 * 64, 1, &q.red)) return 1;
   wgrad_pix_quad_kernel<<<(unsigned)blocks, 256, 0, stream>>>(q);
@@ -1114,10 +1066,7 @@ int launch_wgrad_small(const WgradSimtParams& p, cudaStream_t stream) {
   AB_CHECK(p.npix < (1ll << 32), "wgrad_small: too many pixels");
   AB_CHECK(p.th == TH && p.tw == TW, "wgrad_small: kernel %dx%d != %dx%d", p.th, p.tw, TH, TW);
   const int co_groups = (p.Cout + CO - 1) / CO, ci_groups = (p.S.Ctot + CI - 1) / CI;
-  int64_t bx = (p.npix + 256 * 16 - 1) / (256 * 16);
-  const int64_t cap = (int64_t)ab_num_sms() * 4;
-  if (bx > cap) bx = cap;
-  if (bx < 1) bx = 1;
+  const int64_t bx = ab_grid(p.npix, 256 * 16, 4);
   dim3 grid((unsigned)bx, 1, co_groups * ci_groups);
   WgradSimtParams q = p;
   if (ab_ordered_ws(stream, bx * grid.z * (CO * CI * TH * TW), grid.z, &q.red)) return 1;

@@ -136,8 +136,8 @@ __device__ __forceinline__ void bulk_g2s_if(uint32_t pred, uint32_t dst_smem, co
 // core always has the next group queued.  A streamed weight stage is refilled at that point by
 // the consumer's first thread with the piece it holds next (n_b/2 pieces ahead): the retired group
 // was issued by all four warps, so none of them still waits for the stage's previous contents.
-// PAIR = 2 (resident weights, see ConvTcParams::pair) runs its own pass loop below; the PAIR = 1
-// tile loop is not touched by it.
+// PAIR = 2 (resident weights, see ConvTcParams::pair) runs its own pass loop below and shares the
+// epilogue and the statistics hand-off with the one-tile loop.
 template <int N, int SUB, int PAIR, int PIPE>
 __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* ctl, uint32_t a_base,
                                               uint32_t b_base, float* s_stats, const float* s_bias) {
@@ -194,6 +194,100 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
   }
   constexpr int MB = kTileH / 8;               // m64 row blocks per sub-tile
   float acc[SUB][MB][R];
+
+  // ---------------- epilogue: registers -> bias + activation -> global store + BN statistics
+  const int c_lane = 2 * (lane & 3);
+  // a tile's channel sums, added once the token arrives.  After the butterfly every lane of a
+  // channel pair holds the same sums, so column group j is kept by the lanes with
+  // lane >> 2 == j % 8 only: R / 32 groups per lane instead of R / 4
+  constexpr int JL = (R / 4 + 7) / 8;
+  // tile `tl`'s epilogue from accumulators `a`; `real` = false: the dropped second tile of a
+  // paired pass, which stores nothing.  Its channel sums go to `st` for add_stats.
+  auto epilogue = [&](float (&a)[SUB][MB][R], const int tl, const bool real, float (&st)[JL][4]) {
+    const int n = tl / tpi, rem = tl - n * tpi;
+    const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
+    // compiled once for the plain LeakyReLU and once for every other activation: the per-element
+    // activation switch of the general case, unrolled over the tile, is what the epilogue spilled
+    auto body = [&](auto fast_tag) {
+      constexpr bool FAST = decltype(fast_tag)::value;
+#pragma unroll
+      for (int j = 0; j < R / 4; ++j) {
+        const int c = p.n0 + 8 * j + c_lane;
+        const float b0 = s_bias[c], b1 = s_bias[c + 1];
+        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+        for (int s = 0; s < SUB; ++s)
+#pragma unroll
+          for (int mb = 0; mb < MB; ++mb)
+#pragma unroll
+            for (int hrow = 0; hrow < 2; ++hrow) {
+              const int gh = th_i * kTileH + mb * 8 + 2 * warp + hrow;
+              const int gw = (tw_i * SUB + s) * kTileW + (lane >> 2);
+              const bool valid = real && gh < p.H && gw < p.W;
+              float v0 = a[s][mb][4 * j + 2 * hrow] + b0, v1 = a[s][mb][4 * j + 2 * hrow + 1] + b1;
+              if (FAST) {
+                v0 = fmaxf(v0, v0 * alpha);
+                v1 = fmaxf(v1, v1 * alpha);
+              } else if (p.act == AB_ACT_RBF) {     // alpha * exp(-x/2) as one FMUL + EX2
+                v0 = alpha * exp2f(-0.72134752f * fmaxf(v0, 0.f));
+                v1 = alpha * exp2f(-0.72134752f * fmaxf(v1, 0.f));
+              } else {
+                v0 = act_f(v0, p.act, alpha);
+                v1 = act_f(v1, p.act, alpha);
+              }
+              v0 = valid ? v0 : 0.f;
+              v1 = valid ? v1 : 0.f;
+              if (valid) {
+                const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
+                if (!p.out_nchw) {
+                  *reinterpret_cast<float2*>(p.out + pix * p.ld_out + c) = make_float2(v0, v1);
+                } else {
+                  const size_t hw = (size_t)p.nchw_stride;
+                  float* o = p.out + ((size_t)n * p.Cout + c) * hw + (size_t)gh * p.W + gw;
+                  o[0] = v0;
+                  o[hw] = v1;
+                }
+              }
+              s0 += v0; s1 += v1;
+              q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
+            }
+        if (p.stats) {   // the 8 lanes sharing (lane & 3) hold the same two channels
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+            q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+            q1 += __shfl_xor_sync(0xffffffffu, q1, o);
+          }
+          if ((lane >> 2) == (j & 7)) {
+            st[j >> 3][0] = s0; st[j >> 3][1] = s1; st[j >> 3][2] = q0; st[j >> 3][3] = q1;
+          }
+        }
+      }
+    };
+    if (fast) body(std::true_type{});
+    else body(std::false_type{});
+  };
+  // tile `tl`'s statistics.  Warp w of both consumers adds into s_stats[w] in tile order, as one
+  // consumer did: wait for the other consumer's previous tile, add, pass the token on.  The token
+  // is a named barrier of the two warps (bar.arrive by the passing warp, bar.sync by the waiting
+  // one): a spin on shared memory here puts the next tile's MMAs on a divergent path for ptxas
+  auto add_stats = [&](const int tl, const float (&st)[JL][4]) {
+    if (tl != (int)blockIdx.x) named_bar_sync(kStatBar + (PIPE ? 0 : kNumEpiWarps) + warp, 64);
+#pragma unroll
+    for (int jl = 0; jl < JL; ++jl) {
+      const int j = 8 * jl + (lane >> 2);
+      if (j < R / 4) {
+        const int c = p.n0 + 8 * j + c_lane;
+        my_stats[c] += st[jl][0];
+        my_stats[c + 1] += st[jl][1];
+        my_stats[p.Cout + c] += st[jl][2];
+        my_stats[p.Cout + c + 1] += st[jl][3];
+      }
+    }
+    if (tl + (int)gridDim.x < p.num_tiles)
+      named_bar_arrive(kStatBar + (PIPE ? kNumEpiWarps : 0) + warp, 64);
+  };
 
   auto tile_fn = [&](const int tile) {
     uint32_t pend_a = 0, accum = 0;
@@ -270,97 +364,9 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
     consumer_release(pend_a);
     if (pend_b) refill_b((s_b + nb2 - 1) % nb2, tile + tile_step, 0, 0, (int)nb2 - 1);
 
-    // ---------------- epilogue: registers -> bias + activation -> global store + BN statistics
-    const int n = tile / tpi, rem = tile - n * tpi;
-    const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
-    const int c_lane = 2 * (lane & 3);
-    // this tile's channel sums, added once the token arrives.  After the butterfly every lane of
-    // a channel pair holds the same sums, so column group j is kept by the lanes with
-    // lane >> 2 == j % 8 only: R / 32 groups per lane instead of R / 4
-    constexpr int JL = (R / 4 + 7) / 8;
     float st[JL][4];
-    // compiled once for the plain LeakyReLU and once for every other activation: the per-element
-    // activation switch of the general case, unrolled over the tile, is what the epilogue spilled
-    auto epilogue = [&](auto fast_tag) {
-      constexpr bool FAST = decltype(fast_tag)::value;
-#pragma unroll
-      for (int j = 0; j < R / 4; ++j) {
-        const int cl = 8 * j + c_lane;              // column within this launch
-        const int c = p.n0 + cl;
-        const float b0 = s_bias[c], b1 = s_bias[c + 1];
-        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-#pragma unroll
-        for (int s = 0; s < SUB; ++s)
-#pragma unroll
-          for (int mb = 0; mb < MB; ++mb)
-#pragma unroll
-            for (int hrow = 0; hrow < 2; ++hrow) {
-              const int gh = th_i * kTileH + mb * 8 + 2 * warp + hrow;
-              const int gw = (tw_i * SUB + s) * kTileW + (lane >> 2);
-              const bool valid = gh < p.H && gw < p.W;
-              float v0 = acc[s][mb][4 * j + 2 * hrow] + b0, v1 = acc[s][mb][4 * j + 2 * hrow + 1] + b1;
-              if (FAST) {
-                v0 = fmaxf(v0, v0 * alpha);
-                v1 = fmaxf(v1, v1 * alpha);
-              } else if (p.act == AB_ACT_RBF) {     // alpha * exp(-x/2) as one FMUL + EX2
-                v0 = alpha * exp2f(-0.72134752f * fmaxf(v0, 0.f));
-                v1 = alpha * exp2f(-0.72134752f * fmaxf(v1, 0.f));
-              } else {
-                v0 = act_f(v0, p.act, alpha);
-                v1 = act_f(v1, p.act, alpha);
-              }
-              v0 = valid ? v0 : 0.f;
-              v1 = valid ? v1 : 0.f;
-              if (valid) {
-                const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
-                if (!p.out_nchw) {
-                  *reinterpret_cast<float2*>(p.out + pix * p.ld_out + c) = make_float2(v0, v1);
-                } else {
-                  const size_t hw = (size_t)p.nchw_stride;
-                  float* o = p.out + ((size_t)n * p.Cout + c) * hw + (size_t)gh * p.W + gw;
-                  o[0] = v0;
-                  o[hw] = v1;
-                }
-              }
-              s0 += v0; s1 += v1;
-              q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
-            }
-        if (p.stats) {   // the 8 lanes sharing (lane & 3) hold the same two channels
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-            q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-            q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-          }
-          if ((lane >> 2) == (j & 7)) {
-            st[j >> 3][0] = s0; st[j >> 3][1] = s1; st[j >> 3][2] = q0; st[j >> 3][3] = q1;
-          }
-        }
-      }
-    };
-    if (fast) epilogue(std::true_type{});
-    else epilogue(std::false_type{});
-    if (p.stats) {
-      // warp w of both consumers adds into s_stats[w] in tile order, as one consumer did: wait
-      // for the other consumer's previous tile, add, pass the token on.  The token is a named
-      // barrier of the two warps (bar.arrive by the passing warp, bar.sync by the waiting one): a
-      // spin on shared memory here puts the next tile's MMAs on a divergent path for ptxas
-      if (tile != (int)blockIdx.x) named_bar_sync(kStatBar + (PIPE ? 0 : kNumEpiWarps) + warp, 64);
-#pragma unroll
-      for (int jl = 0; jl < JL; ++jl) {
-        const int j = 8 * jl + (lane >> 2);
-        if (j < R / 4) {
-          const int c = p.n0 + 8 * j + c_lane;
-          my_stats[c] += st[jl][0];
-          my_stats[c + 1] += st[jl][1];
-          my_stats[p.Cout + c] += st[jl][2];
-          my_stats[p.Cout + c + 1] += st[jl][3];
-        }
-      }
-      if (tile + (int)gridDim.x < p.num_tiles)
-        named_bar_arrive(kStatBar + (PIPE ? kNumEpiWarps : 0) + warp, 64);
-    }
+    epilogue(acc, tile, true, st);
+    if (p.stats) add_stats(tile, st);
   };
 
   if constexpr (PAIR == 1) {
@@ -374,91 +380,7 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
     // no MMA or wgmma wait depends on whether the pass has two tiles.  Both tiles' epilogues run
     // before the first statistics add: accumulators read after the lane-dependent adds also
     // serialise the MMAs.
-    constexpr int JL = (R / 4 + 7) / 8;
-    const int c_lane = 2 * (lane & 3);
     float pacc[2][SUB][MB][R];
-    // tile `tl`'s epilogue from accumulators `a`, as tile_fn's; `real` = 0: the dropped second
-    // tile, which stores nothing.  Its channel sums go to `st` for add_stats.
-    auto pair_epilogue = [&](float (&a)[SUB][MB][R], const int tl, const bool real, float (&st)[JL][4]) {
-      const int n = tl / tpi, rem = tl - n * tpi;
-      const int th_i = rem / p.tiles_w, tw_i = rem - th_i * p.tiles_w;
-      auto epilogue = [&](auto fast_tag) {
-        constexpr bool FAST = decltype(fast_tag)::value;
-#pragma unroll
-        for (int j = 0; j < R / 4; ++j) {
-          const int c = p.n0 + 8 * j + c_lane;
-          const float b0 = s_bias[c], b1 = s_bias[c + 1];
-          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-#pragma unroll
-          for (int s = 0; s < SUB; ++s)
-#pragma unroll
-            for (int mb = 0; mb < MB; ++mb)
-#pragma unroll
-              for (int hrow = 0; hrow < 2; ++hrow) {
-                const int gh = th_i * kTileH + mb * 8 + 2 * warp + hrow;
-                const int gw = (tw_i * SUB + s) * kTileW + (lane >> 2);
-                const bool valid = real && gh < p.H && gw < p.W;
-                float v0 = a[s][mb][4 * j + 2 * hrow] + b0, v1 = a[s][mb][4 * j + 2 * hrow + 1] + b1;
-                if (FAST) {
-                  v0 = fmaxf(v0, v0 * alpha);
-                  v1 = fmaxf(v1, v1 * alpha);
-                } else if (p.act == AB_ACT_RBF) {
-                  v0 = alpha * exp2f(-0.72134752f * fmaxf(v0, 0.f));
-                  v1 = alpha * exp2f(-0.72134752f * fmaxf(v1, 0.f));
-                } else {
-                  v0 = act_f(v0, p.act, alpha);
-                  v1 = act_f(v1, p.act, alpha);
-                }
-                v0 = valid ? v0 : 0.f;
-                v1 = valid ? v1 : 0.f;
-                if (valid) {
-                  const size_t pix = ((size_t)n * p.H + gh) * p.W + gw;
-                  if (!p.out_nchw) {
-                    *reinterpret_cast<float2*>(p.out + pix * p.ld_out + c) = make_float2(v0, v1);
-                  } else {
-                    const size_t hw = (size_t)p.nchw_stride;
-                    float* o = p.out + ((size_t)n * p.Cout + c) * hw + (size_t)gh * p.W + gw;
-                    o[0] = v0;
-                    o[hw] = v1;
-                  }
-                }
-                s0 += v0; s1 += v1;
-                q0 = fmaf(v0, v0, q0); q1 = fmaf(v1, v1, q1);
-              }
-          if (p.stats) {
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) {
-              s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-              s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-              q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-              q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-            }
-            if ((lane >> 2) == (j & 7)) {
-              st[j >> 3][0] = s0; st[j >> 3][1] = s1; st[j >> 3][2] = q0; st[j >> 3][3] = q1;
-            }
-          }
-        }
-      };
-      if (fast) epilogue(std::true_type{});
-      else epilogue(std::false_type{});
-    };
-    // tile `tl`'s statistics, added in tile order as tile_fn does
-    auto add_stats = [&](const int tl, const float (&st)[JL][4]) {
-      if (tl != (int)blockIdx.x) named_bar_sync(kStatBar + (PIPE ? 0 : kNumEpiWarps) + warp, 64);
-#pragma unroll
-      for (int jl = 0; jl < JL; ++jl) {
-        const int j = 8 * jl + (lane >> 2);
-        if (j < R / 4) {
-          const int c = p.n0 + 8 * j + c_lane;
-          my_stats[c] += st[jl][0];
-          my_stats[c + 1] += st[jl][1];
-          my_stats[p.Cout + c] += st[jl][2];
-          my_stats[p.Cout + c + 1] += st[jl][3];
-        }
-      }
-      if (tl + (int)gridDim.x < p.num_tiles)
-        named_bar_arrive(kStatBar + (PIPE ? kNumEpiWarps : 0) + warp, 64);
-    };
     auto pass_fn = [&](const int tile) {
       const bool two = tile + tile_step < p.num_tiles;
       uint32_t accum = 0;
@@ -515,7 +437,7 @@ __device__ __forceinline__ void consumer_loop(const ConvTcParams& p, SharedCtl* 
           for (int mb = 0; mb < MB; ++mb) wgmma_fence_regs(pacc[w][s][mb]);
       float st[2][JL][4];
 #pragma unroll
-      for (int w = 0; w < 2; ++w) pair_epilogue(pacc[w], tile + w * tile_step, w == 0 || two, st[w]);
+      for (int w = 0; w < 2; ++w) epilogue(pacc[w], tile + w * tile_step, w == 0 || two, st[w]);
       if (p.stats) {
         add_stats(tile, st[0]);
         if (two) add_stats(tile + tile_step, st[1]);
@@ -597,15 +519,12 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
   const float inv_tpi = 1.f / (float)tpi, inv_tw = 1.f / (float)p.tiles_w;
   const int n_chunks = p.n_chunks;
   const uint32_t n_a = p.n_a;
-  // Streamed weights: one pipeline, group g stages the chunks with (running counter & 1) == g.
-  // Resident weights (dual pipelines): group g stages every chunk of the tiles with local index
-  // = g (mod 2) into its own half of the stage ring.
-  const bool dual = true;   // both weight modes run two pipelines (group g -> issuer g)
-  const int ch_step = dual ? 1 : 2;
-  const int tile_step = dual ? 2 * gridDim.x : gridDim.x;
-  const uint32_t ring_n = dual ? n_a / 2 : n_a;
-  const uint32_t ring0 = dual ? grp * ring_n : 0u;
-  int tile = dual ? blockIdx.x + grp * gridDim.x : blockIdx.x;
+  // group g stages every chunk of the tiles with CTA-local index = g (mod 2) into its own half of
+  // the stage ring, for consumer g
+  const int tile_step = 2 * gridDim.x;
+  const uint32_t ring_n = n_a / 2;
+  const uint32_t ring0 = grp * ring_n;
+  int tile = blockIdx.x + grp * gridDim.x;
   // PAIR = 2: a pass covers the group's tiles `tile` and tile + tile_step, k-chunk by k-chunk in
   // the order its consumer takes them: pass chunk ch is k-chunk ch / 2 of the pass's tile ch % 2
   // (`tile` again when tile + tile_step is past the end)
@@ -650,9 +569,8 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
       if (r_tile < p.num_tiles) issue_raw(tile_of(r_tile, r_ch), r_ch / PAIR, i);
     }
   }
-  int ch = dual ? 0 : grp;
-  uint32_t st = dual ? 0u : grp % n_a;
-  uint32_t ph = dual ? 1u : ((grp / n_a) & 1) ^ 1;   // stage / empty-phase of the current chunk
+  int ch = 0;
+  uint32_t st = 0, ph = 1;   // stage / empty-phase of the current chunk
   for (;;) {
     while (ch >= n_chunks_eff) { ch -= n_chunks_eff; tile += PAIR * tile_step; }
     if (tile >= p.num_tiles) break;
@@ -833,9 +751,8 @@ __device__ __forceinline__ void loader_loop(const ConvTcParams& p, SharedCtl* ct
       if (++rst == rn) { rst = 0; rph ^= 1; }
     }
     // advance to this group's next chunk
-    ch += ch_step;
-    st += ch_step;
-    while (st >= ring_n) { st -= ring_n; ph ^= 1; }
+    ++ch;
+    if (++st == ring_n) { st = 0; ph ^= 1; }
   }
 }
 
